@@ -1,9 +1,9 @@
 #!/bin/bash
-# Build libb200z.so (sm_100a only) and the corpus helper in-tree.  Usage: ./build.sh [-v]
+# Build libb200z.so (sm_90a only) and the corpus helper in-tree.  Usage: ./build.sh [-v]
 set -e
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC -Icsrc -I../include"
+FLAGS="-O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC -Icsrc -I../include"
 [ "$1" = "-v" ] && FLAGS="$FLAGS -Xptxas -v"
 mkdir -p build
 objs=""
@@ -17,7 +17,7 @@ for f in csrc/*.cu; do
   objs="$objs $o"
 done
 for p in $pids; do wait $p || { echo "build.sh: compilation FAILED" >&2; exit 1; }; done
-$NVCC -shared -gencode arch=compute_100a,code=sm_100a -o libb200z.so $objs -lcudart
+$NVCC -shared -gencode arch=compute_90a,code=sm_90a -o libb200z.so $objs -lcudart
 gcc -O2 -shared -fPIC -pthread -o corpus/libb200z_corpus.so corpus/g2gen.c
 # 7-Zip codec module (ICompressCoder classes + CodecExports) and its C++ test driver
 g++ -std=c++17 -O2 -fPIC -shared -Wall -Wno-misleading-indentation codec/ZstdCoders.cpp codec/Lzma2Coders.cpp -I../include -L. -lb200z -Wl,-rpath,'$ORIGIN' -o libb200z_7z.so

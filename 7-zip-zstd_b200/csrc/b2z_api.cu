@@ -324,7 +324,7 @@ static int enc_batch(b200z_ctx* ctx, const uint8_t* d_src, uint64_t n, uint8_t* 
         cudaEventElapsedTime(&ms, ctx->ev[2], ctx->ev[3]); ctx->stat[B200Z_S_ENC_ASSEMBLE_MS] += ms;
     } else if (!stageMOnly) {
         launch_zstd_enc_entropy(d_src, n, g, (const uint64_t*)ctx->seqs.p, (const uint32_t*)ctx->nseq.p, (const uint8_t*)ctx->lits.p,
-                                (const uint32_t*)ctx->nlit.p, (uint8_t*)ctx->slots.p, (uint32_t*)ctx->slotSize.p, nBlocks, st);
+                                (const uint32_t*)ctx->nlit.p, (uint8_t*)ctx->slots.p, (uint32_t*)ctx->slotSize.p, nBlocks, ctx->smCount, st);
         CU(cudaGetLastError());
         CU(cudaEventRecord(ctx->ev[2], st));
         launch_zstd_enc_assemble(d_src, n, g, (const uint8_t*)ctx->slots.p, (const uint32_t*)ctx->slotSize.p, nBlocks, (uint64_t*)ctx->blockOff.p,
@@ -469,7 +469,7 @@ int b200z_zstd_compress_host(b200z_ctx* ctx, const void* src, size_t srcSize, vo
         if (per < batch) batch = per;
     }
     if (batch < F) batch = F;
-    {   // whole rounds of stage F's grid (one CTA per SM, one region each): a batch of 1024 regions would end with a round of 136 of 148 CTAs
+    {   // whole rounds of stage F's grid (one CTA per SM, one region each): a batch of 1024 regions would end with a partial round (1024 = 7 x 132 + 100 on an H100)
         const uint64_t unit = long_mode(ctx->geom, 0) ? 1ull << ctx->geom.regionLog : F, round = (uint64_t)ctx->smCount * unit;
         if (!(ctx->geom.flags & B2Z_FLAG_ZSTD_OPT) && batch > round && srcSize > batch) { const uint64_t b = batch / round * round; if (b % F == 0) batch = b; }
     }

@@ -1,4 +1,4 @@
-// b2z_crc.cu -- CRC32 and CRC64 of device buffers (sm_100a): the digests the archive layer computes over every byte next to the
+// b2z_crc.cu -- CRC32 and CRC64 of device buffers (sm_90a): the digests the archive layer computes over every byte next to the
 // coders -- 7-Zip's CRC32 of each file / folder (C/7zCrc.c:298 CrcCalc, CPP/7zip/Common/InStreamWithCRC.cpp) and xz's CRC64 block
 // check (C/XzCrc64.c, C/Xz.h:34 XZ_CHECK_CRC64).  SURVEY.md 8(f) item 4: once the coder is fast the host's CRC is the bottleneck.
 //

@@ -29,14 +29,14 @@ struct b200z_ctx {
     cudaStream_t stream2 = nullptr;   // side stream (decoder: literals kernel next to the sequences kernel; host path: uploads)
     cudaStream_t stream3 = nullptr;   // host path: downloads
     cudaEvent_t pe[4] = {};           // host-path pipeline events
-    uint32_t hostBatchLog = 30;       // bytes per pipeline batch of the host-pointer entry points: 1 GiB = 1024 frames = 7 rounds of
-                                      // stage F's one-CTA-per-SM grid, so H2D | kernels | D2H of consecutive batches overlap.  The decoder
+    uint32_t hostBatchLog = 30;       // bytes per pipeline batch of the host-pointer entry points: up to 1 GiB, trimmed to whole rounds of stage F's
+                                      // one-CTA-per-SM grid (924 frames = 7 rounds on 132 SMs), so H2D | kernels | D2H of consecutive batches overlap.  The decoder
                                       // (one warp per frame in its execute stage) takes batches twice as large
     b2z::EncGeom geom{};
     int level = 3;
     uint32_t batchLog = 31;           // bytes per kernel batch of the device-pointer entry points: 2 GiB keeps the scratch (9.5 bytes per batch byte: candidate
-                                      // words 4, choices 1, sequences 2, literals 1, block slots 1.5) near 19 GiB whatever the input size (1 GiB batches cost 4 % of speed)
-    uint32_t smCount = 148;
+                                      // words 4, choices 1, sequences 2, literals 1, block slots 1.5) near 19 GiB whatever the input size
+    uint32_t smCount = 132;           // replaced by the device's count in b200z_create
     uint32_t decJumpSegLog = B2Z_DEC_JUMP_SEGLOG;   // stage J: bytes of output resolved per pass (B200Z_P_DEC_JUMP_SEGLOG; tests use small segments)
     int decJump = 1;                  // Zstandard decoder, stage J (frames resolved by pointer jumping): 0 never, 1 frames whose units form a chain, 2 every frame
     int lz2Mode = 0;                  // LZMA2 decoder literal-model placement: 0 auto, 1 shared memory, 2 global memory

@@ -71,7 +71,7 @@ void launch_zstd_dec_index_blocks(const uint8_t* src, uint64_t srcSize, DecFrame
                                   DecBlock* blocks, uint32_t blockCap, DecCounts* counts, cudaStream_t st);
 // stage D1: tables (one warp per block) then streams (one thread per stream); literals | sequences on two CUDA streams
 void launch_zstd_dec_entropy(const uint8_t* src, uint64_t srcSize, DecBlock* blocks, uint32_t nBlocks,
-                             uint8_t* lits, uint64_t* seqs, void* scratch, cudaStream_t st, cudaStream_t stLit, cudaEvent_t evFork, cudaEvent_t evJoin);
+                             uint8_t* lits, uint64_t* seqs, void* scratch, uint32_t smCount, cudaStream_t st, cudaStream_t stLit, cudaEvent_t evFork, cudaEvent_t evJoin);
 size_t zstd_dec_entropy_scratch_bytes(uint32_t nBlocks);
 // stage D2: per-frame sizes and output offsets
 // jumpMode: 0 = every frame by units (stage D3), 1 = frames whose units form a chain go to stage J, 2 = every frame with a block goes to stage J
@@ -81,12 +81,12 @@ void launch_zstd_dec_layout(DecFrame* frames, uint32_t nFrames, DecBlock* blocks
 // scratch: zstd_dec_jump_scratch_bytes(total, segLog) -- round flags, one word per output byte of a segment, one byte per 128 of them
 size_t zstd_dec_jump_scratch_bytes(uint64_t total, uint32_t segLog /* <= B2Z_DEC_JUMP_SEGLOG */);
 void launch_zstd_dec_jump(const uint8_t* src, DecFrame* frames, uint32_t nFrames, DecBlock* blocks, uint32_t nBlocks, const uint8_t* lits, const uint64_t* seqs,
-                          uint8_t* dst, uint64_t total, uint32_t segLog, DecCounts* counts, void* scratch, cudaStream_t st);
+                          uint8_t* dst, uint64_t total, uint32_t segLog, DecCounts* counts, void* scratch, uint32_t smCount, cudaStream_t st);
 // stage D3: one warp per unit of B2Z_DEC_UNIT_BLOCKS consecutive blocks of a frame, units taken in order; a match that reaches
 // behind its unit waits for the unit that writes those bytes.  unitState: [0] ticket, [1 + u] done flag of unit u -- zeroed here.
 size_t zstd_dec_unit_state_bytes(uint32_t nFrames, uint32_t nBlocks);
 void launch_zstd_dec_exec(const uint8_t* src, DecFrame* frames, uint32_t nFrames, DecBlock* blocks, uint32_t nBlocks,
-                          const uint8_t* lits, const uint64_t* seqs, uint8_t* dst, DecCounts* counts, uint32_t* unitState, cudaStream_t st);
+                          const uint8_t* lits, const uint64_t* seqs, uint8_t* dst, DecCounts* counts, uint32_t* unitState, uint32_t smCount, cudaStream_t st);
 
 // content checksums (XXH64 low 32 bits) of the frames that carry one: one thread per frame, after D3
 void launch_zstd_dec_verify(const uint8_t* src, const DecFrame* frames, uint32_t nFrames, const uint8_t* dst, DecCounts* counts, cudaStream_t st);

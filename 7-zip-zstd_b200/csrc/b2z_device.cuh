@@ -1,4 +1,4 @@
-// b2z_device.cuh -- small device helpers shared by the sm_100a kernels.
+// b2z_device.cuh -- small device helpers shared by the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -157,7 +157,7 @@ __device__ inline uint64_t xxh64_device_unaligned(const uint8_t* data, uint64_t 
 
 
 // XXH64 by one warp, for the one big frame the reference's .zst handler writes with a content checksum (ZstdHandler.cpp:262-282).
-// The four stripe accumulators are four strictly sequential chains -- lanes 0-3 run one each, ~25 cycles of dependent 64-bit
+// The four stripe accumulators are four strictly sequential chains -- lanes 0-3 run one each, dependent 64-bit
 // arithmetic per 32 input bytes, which is the floor for this hash on any machine that cannot multiply faster.  What the other lanes
 // add is the memory pipeline: the warp loads the next tile (aligned 16-byte words, coalesced, any byte alignment of `data`) into
 // registers while the four lanes work on the current one from shared memory.  tileMem: 2 * B2Z_XXH_TILE_BYTES, 16-byte aligned.

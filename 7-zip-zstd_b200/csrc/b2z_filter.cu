@@ -170,7 +170,7 @@ int b2z_filter_units_device(b200z_ctx* ctx, uint32_t methodId, int encode, void*
         if (nHalf >= 2) {
             if (ctx->batchStage.reserve(n)) return fail(ctx, B200Z_E_MEMORY, "device scratch allocation failed%s");
             CU(cudaMemcpyAsync(ctx->batchStage.p, d_data, n, cudaMemcpyDeviceToDevice, st));
-            b2z::armt_kernel<<<(unsigned)((nHalf + 255) / 256 < 148u * 64u ? (nHalf + 255) / 256 : 148u * 64u), 256, 0, st>>>((const uint16_t*)ctx->batchStage.p, (uint16_t*)d_data, nHalf, encode, prop, unitLog);
+            b2z::armt_kernel<<<(unsigned)((nHalf + 255) / 256 < ctx->smCount * 64u ? (nHalf + 255) / 256 : ctx->smCount * 64u), 256, 0, st>>>((const uint16_t*)ctx->batchStage.p, (uint16_t*)d_data, nHalf, encode, prop, unitLog);
             ctx->stat[B200Z_S_KERNEL_LAUNCHES] += 1;
         }
     } else if (methodId == B200Z_F_ARM64 || methodId == B200Z_F_ARM || methodId == B200Z_F_PPC || methodId == B200Z_F_SPARC) {
@@ -178,7 +178,7 @@ int b2z_filter_units_device(b200z_ctx* ctx, uint32_t methodId, int encode, void*
         if (prop & 3u) return fail(ctx, B200Z_E_UNSUPPORTED, "start offset must be a multiple of the instruction size%s");   // BranchMisc.cpp:57,99: E_INVALIDARG / E_NOTIMPL
         const uint64_t nWords = n >> 2;
         if (!nWords) return 0;
-        b2z::bra_kernel<<<(unsigned)((nWords + 255) / 256 < 148u * 64u ? (nWords + 255) / 256 : 148u * 64u), 256, 0, st>>>((uint32_t*)d_data, nWords, methodId, encode, prop, unitLog);
+        b2z::bra_kernel<<<(unsigned)((nWords + 255) / 256 < ctx->smCount * 64u ? (nWords + 255) / 256 : ctx->smCount * 64u), 256, 0, st>>>((uint32_t*)d_data, nWords, methodId, encode, prop, unitLog);
         ctx->stat[B200Z_S_KERNEL_LAUNCHES] += 1;
     } else return fail(ctx, B200Z_E_UNSUPPORTED, "filter not built on the GPU (BCJ2 / RISCV / IA64)%s");
     CU(cudaGetLastError());

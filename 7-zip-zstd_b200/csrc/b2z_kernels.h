@@ -1,4 +1,4 @@
-// b2z_kernels.h -- host-visible launchers of the sm_100a kernels (internal to libb200z.so).
+// b2z_kernels.h -- host-visible launchers of the sm_90a kernels (internal to libb200z.so).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -45,7 +45,7 @@ cudaError_t launch_zstd_enc_parse(const uint8_t* src, uint64_t srcSize, const En
 // stage E: one warp per 128 KiB block -> compressed block (with 3-byte header) in its slot
 void launch_zstd_enc_entropy(const uint8_t* src, uint64_t srcSize, const EncGeom& g,
                              const uint64_t* seqs, const uint32_t* nseq, const uint8_t* lits, const uint32_t* nlit,
-                             uint8_t* slots, uint32_t* slotSize, uint32_t nBlocks, cudaStream_t st);
+                             uint8_t* slots, uint32_t* slotSize, uint32_t nBlocks, uint32_t smCount, cudaStream_t st);
 
 // frame assembly: offsets (one CTA scan) + gather of slots into contiguous frames
 void launch_zstd_enc_assemble(const uint8_t* src, uint64_t srcSize, const EncGeom& g, const uint8_t* slots, const uint32_t* slotSize,

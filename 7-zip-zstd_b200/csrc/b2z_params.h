@@ -37,7 +37,7 @@
  * position in 2^B2Z_LDM_RATELOG, for the first place of the frame that holds the same B2Z_LDM_MINMATCH bytes */
 #define B2Z_DEF_PLAIN_REGIONLOG 19  /* outside the long mode: a 1 MiB frame is two regions.  Costs 0.2 % of ratio on text (2.3825 -> 2.3777: the
                                     * second region starts with empty tables) and halves the longest chain the decoder's execute stage has to
-                                    * walk (its units are 4 blocks): host-to-host decode of 4 GiB 143 -> 128 ms */
+                                    * walk (its units are 4 blocks) */
 #define B2Z_MAX_LONGLOG    27
 #define B2Z_DEF_REGIONLOG  20
 #define B2Z_LDM_MINMATCH   64u

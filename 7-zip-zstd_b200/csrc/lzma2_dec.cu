@@ -1,4 +1,4 @@
-// lzma2_dec.cu -- block-parallel LZMA2 decoder (7-Zip method 21) for sm_100a.
+// lzma2_dec.cu -- block-parallel LZMA2 decoder (7-Zip method 21) for sm_90a.
 //
 // Pre-pass  lzma2_walk_kernel    one thread hops over the chunk headers (<= 64 KiB of payload per hop) and cuts
 //                                the stream at dictionary resets -> Lz2Block[] with output offsets.

@@ -1,15 +1,15 @@
-// lzma2_enc.cu -- stage R of the block-parallel LZMA2 encoder (7-Zip method 21) for sm_100a.
+// lzma2_enc.cu -- stage R of the block-parallel LZMA2 encoder (7-Zip method 21) for sm_90a.
 //
 // A frame (2^frameLog input bytes) becomes one dictionary-reset LZMA2 block -- the independent unit the reference's own
 // MT coders use (Lzma2Enc.c:241-330 block split; fast-lzma2 slices, lzma2_enc.c:1937-2099).  Stage M (zstd_enc_match.cu,
 // shared with the zstd path) -- or, with B2Z_FLAG_LZ2_OPT, stage C + stage P (lzma2_parse.cu: the price-based parse) -- has
 // already found the frame's sequences; here one thread per frame codes them as LZMA
-// packets with the adaptive binary range coder, which is a strictly serial chain of ~100 instructions per input byte:
+// packets with the adaptive binary range coder, which is a strictly serial chain of dependent instructions:
 // the parallelism is across frames (thousands per batch), not inside one.
 //   model      11-bit probabilities in shared memory (16 KiB, 13 frames/SM) or, when there are more frames than that
 //              fills, the 12 KiB literal part in global memory (32 frames/SM)
 //   input      bytes the next packet needs (its symbol, the previous byte, the byte at rep0) are loaded before the
-//              current packet is coded, so their L2 latency hides under ~10^3 cycles of range coding
+//              current packet is coded, so their L2 latency hides under the range coding of the current one
 //   chunks     closed at 64 KiB - 64 packed bytes or 2 MiB - 512 covered; a chunk that does not shrink is rewritten as
 //              an uncompressed chunk and the next one resets the model (Lzma2Enc.c:183-238)
 //
@@ -30,7 +30,7 @@ struct RcE {
 };
 
 // Not inlined on purpose: it runs once per ~13 coded bits, and inlining it at the ~25 rce_bit sites (with its byte loop
-// unrolled) made the kernel 145 KB of SASS -- ncu showed 1.2 "no instruction" stall cycles per issue (i-cache misses).
+// unrolled) made the kernel large enough to miss in the instruction cache.
 __device__ __noinline__ void rce_shift_low(RcE& e) {
     if ((uint32_t)e.low < 0xFF000000u || (uint32_t)(e.low >> 32) != 0u) {
         const uint32_t carry = (uint32_t)(e.low >> 32);
@@ -73,8 +73,8 @@ __device__ __forceinline__ void rce_len(RcE& e, uint16_t* l, uint32_t len, uint3
     else { rce_bit(e, l + L_CHOICE, 1); rce_bit(e, l + L_CHOICE2, 1); rce_tree(e, l + L_HIGH, 8, len - 16u); }
 }
 
-// L: chains per warp (lanes 0, 32/L, 2*32/L ... each run one chain).  Only L = 1 is launched: measured on 4 GiB, L = 2/4/8
-// take 1566/1952/2007 ms against 836 ms -- the chains' control flow diverges at every coded bit, so the hardware
+// L: chains per warp (lanes 0, 32/L, 2*32/L ... each run one chain).  Only L = 1 is launched: L = 2/4/8 measured
+// slower -- the chains' control flow diverges at every coded bit, so the hardware
 // serialises them and the shared convergent code does not pay for it.
 template <bool GLIT, int L>
 // <= 64 registers: they are allocated for all 32 lanes of a chain's warp, so registers -- not shared memory -- bound the
@@ -251,15 +251,10 @@ lzma2_enc_range_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
 //           the probabilities -- until the queue holds B2Z_R32_FILL decisions;
 //   phase B (lock-step): B2Z_R32_FILL times, all 32 lanes pop a decision and code it.  The probabilities of the steps to come are loaded
 //           B2Z_R32_DEPTH steps ahead (a step that adapts one of them marks the slot stale; a stale slot loads again at its turn).
-// STATUS: parity-green on B200 (bytes of the kernel above) but not the default: 1.9 s per 4 GiB against 0.98 s for one chain per warp.
-// Why, in numbers (profiles/r2_range32_ncu.txt): the warp executes ~185 instructions per step of 32 decisions -- 6 per decision where the
-// single-chain kernel spends 30 -- so the whole job is 4x fewer instructions.  But the single-chain kernel is ISSUE-bound (32 resident warps
-// per SM keep the schedulers at 0.7 instructions per cycle), while 16 384 chains are only 512 lock-step warps, 3.5 per SM, each issuing one
-// instruction per ~6-7 cycles (dependent arithmetic, shared-memory and L1/L2 latencies, nothing else to run): chip-wide 11 decisions per cycle
-// against 34.  A third version that gathered a round's distinct probabilities into a shared-memory hash table with all their loads in flight
-// at once and prefetched the producer's input bytes removed the DRAM waits and was no faster (2.2 s: 229 instructions per step) -- the bound
-// is instructions per step x latency per instruction at this warp count, not memory.  Lock-step pays only with >= ~24 such warps per SM, i.e.
-// ~100 000 chains (slices of ~40 KiB: a ratio cost nobody wants), or below ~75 instructions per step.  Selected with B200Z_P_LZMA2_MODEL = 3.
+// STATUS: parity-green (bytes of the kernel above) but not the default: it was slower than one chain per warp.
+// Why: it executes far fewer instructions per decision, but 16 384 chains are only 512 lock-step warps, a handful per SM, each waiting on
+// its own dependent latencies with nothing else to run, while the single-chain kernel is issue-bound with many warps per SM.  Selected with
+// B200Z_P_LZMA2_MODEL = 3.
 // The models live in global memory, interleaved by lane (probability i of lane l at [i][l]).  Chunk rules are the single-chain kernel's:
 // a packet may be queued ahead of its coding only while the chunk cannot reach its packed limit before it (a decision emits at most one
 // byte, so `packed + queued < limit` is a proof); near the limit a lane queues one packet at a time and decides with an empty queue, which
@@ -424,7 +419,7 @@ lzma2_enc_range32_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncG
     for (;;) {
         // ---- phase A: queue packets until B2Z_R32_FILL decisions wait (or the lane has to see its queue drain first).  Every pass of the
         // loop is one packet per lane; the __syncwarp()s are there for the hardware, not for the data: without a convergence point after
-        // each section the lanes drift apart and the warp executes them one after the other (measured: 2.4 s per 4 GiB, the cost of 32
+        // each section the lanes drift apart and the warp executes them one after the other (the cost of 32
         // serial chains)
         bool blocked = false;
         for (;;) {
@@ -552,8 +547,8 @@ cudaError_t launch_lzma2_enc_range(const uint8_t* src, uint64_t srcSize, const E
     const uint32_t nChains = nFrames * lzma2_enc_slices_per_frame(g);
     const size_t smemFull = ((size_t)P_LIT + LITN) * sizeof(uint16_t);
     const uint32_t slotsResident = (uint32_t)((227u * 1024u) / (smemFull + 1024)) * smCount;
-    // Measured (4 GiB, 16384 chains): literal model in global memory, 60 chains per SM: 903 ms; whole model in shared memory
-    // (9.6 KiB at lc = 2, 23 chains per SM): 1226 ms -- residency beats the ~6 extra instructions per literal bit.
+    // Literal model in global memory when the chains outnumber the shared-memory slots: more chains resident beat the ~6 extra
+    // instructions per literal bit of the global-memory model.
     const bool glit = mode == 2 || (mode == 0 && litSpill && nChains > slotsResident);
     const uint32_t stride = (uint32_t)lzma2_enc_slot_stride(g);
     if (mode == 3) {                                                // 32 chains per warp (experimental, see the kernel's header); litSpill holds whole models here (lzma2_enc_model_bytes)

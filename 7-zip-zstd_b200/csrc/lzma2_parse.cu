@@ -1,4 +1,4 @@
-// lzma2_parse.cu -- the price-based parse of the block-parallel LZMA2 encoder (7-Zip method 21, flag B2Z_FLAG_LZ2_OPT) for sm_100a.
+// lzma2_parse.cu -- the price-based parse of the block-parallel LZMA2 encoder (7-Zip method 21, flag B2Z_FLAG_LZ2_OPT) for sm_90a.
 //
 // Two kernels in front of stage R (lzma2_enc.cu), replacing the greedy stage M for this mode:
 //

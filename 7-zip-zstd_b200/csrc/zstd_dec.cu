@@ -1,4 +1,4 @@
-// zstd_dec.cu -- Zstandard decoder kernels (sm_100a), bit-exact for any valid frame whose
+// zstd_dec.cu -- Zstandard decoder kernels (sm_90a), bit-exact for any valid frame whose
 // window is <= 2^29 and that needs no dictionary.
 //
 //   D0 prepass  (1 thread)          walk frame and block headers (sequential by format), record
@@ -614,7 +614,7 @@ zstd_dec_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, DecBl
 
 // ---------------------------------------------------------------- D1b: one thread per stream
 // Literal streams.  The decoding tables (up to 4 KiB per block, 128 MB for the 32 768 blocks of 4 GiB) do not fit L2 while every stream
-// of the input is in flight, and a look-up per symbol from HBM was what this kernel waited for (26.6 ms per 4 GiB).  A CTA therefore
+// of the input is in flight, and a look-up per symbol from HBM was what this kernel waited for.  A CTA therefore
 // serves LIT_BLOCKS blocks (4 streams each) and first copies their tables into shared memory: the per-symbol chain is then two shifts,
 // one shared-memory load and an add.
 #define B2Z_LIT_BLOCKS 16u
@@ -757,7 +757,8 @@ zstd_dec_seq_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
 // jumpMode (b2z_dec.h): which frames leave the execution units for stage J.  Automatic: a frame of >= B2Z_DEC_JUMP_MIN_UNITS units in which
 // three consecutive units (or three in four of all) start with a block that copies from the unit before it -- a sliding-window frame (what
 // the reference's encoder writes: one frame per stream, ZstdEncoder.cpp:250-340), whose units would run one behind the other.  The test is
-// deliberately easy to pass: a frame taken by stage J for nothing costs ~35 ms per GiB instead of ~4, a chain left to the units ~12 s per GiB
+// deliberately easy to pass: a frame taken by stage J for nothing costs several times the units' time, a chain left to the units
+// orders of magnitude more
 // (binaries compressed at level >= 3 split their blocks and copy by repcodes: only two units in three show the dependency in their first block).
 __global__ void zstd_dec_frame_sizes_kernel(DecFrame* frames, uint32_t nFrames, DecBlock* __restrict__ blocks, DecCounts* counts, uint32_t jumpMode) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1203,7 +1204,7 @@ void launch_zstd_dec_index_blocks(const uint8_t* src, uint64_t srcSize, DecFrame
     zstd_dec_fill_blocks_kernel<<<grid, 64, 0, st>>>(src, srcSize, frames, nFrames, blocks, blockCap, counts);
 }
 void launch_zstd_dec_entropy(const uint8_t* src, uint64_t srcSize, DecBlock* blocks, uint32_t nBlocks, uint8_t* lits, uint64_t* seqs,
-                             void* scratch, cudaStream_t st, cudaStream_t stLit, cudaEvent_t evFork, cudaEvent_t evJoin) {
+                             void* scratch, uint32_t smCount, cudaStream_t st, cudaStream_t stLit, cudaEvent_t evFork, cudaEvent_t evJoin) {
     if (!nBlocks) return;
     // scratch layout: hufTabs [nBlocks][2048] u16 | seqTabs [nBlocks][1280] SeqEnt | litJobs | seqJobs
     uint8_t* p = (uint8_t*)scratch;
@@ -1212,15 +1213,16 @@ void launch_zstd_dec_entropy(const uint8_t* src, uint64_t srcSize, DecBlock* blo
     LitJob* litJobs = (LitJob*)p; p += (size_t)nBlocks * sizeof(LitJob);
     SeqJob* seqJobs = (SeqJob*)p;
     // The literal and the sequence kernels only read src/blocks and write disjoint outputs, so they may run on two streams
-    // (stLit != st).  Measured on B200 (2 GiB, repeated calls): one stream 30.5 ms, two streams 46 ms -- every call after
-    // the first one; the four kernels each fill the GPU and co-scheduling them only makes them evict each other's lines.
+    // (stLit != st).  The four kernels each fill the GPU, and co-scheduling them
+    // only makes them evict each other's lines (two streams measured slower than one).
     // The host dispatcher therefore passes stLit == st.
     if (stLit != st) { cudaEventRecord(evFork, st); cudaStreamWaitEvent(stLit, evFork, 0); }
-    { uint32_t grid = (nBlocks + D1_WARPS(0) - 1) / D1_WARPS(0); if (grid > 148u * 16u) grid = 148u * 16u;
+    const uint32_t cap = smCount * 16u;
+    { uint32_t grid = (nBlocks + D1_WARPS(0) - 1) / D1_WARPS(0); if (grid > cap) grid = cap;
       zstd_dec_entropy_kernel<0><<<grid, D1_WARPS(0) * 32, 0, stLit>>>(src, srcSize, blocks, nBlocks, lits, hufTabs, litJobs, seqTabs, seqJobs);
       cudaFuncSetAttribute(zstd_dec_lit_streams_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(B2Z_LIT_BLOCKS * 4096u));
       zstd_dec_lit_streams_kernel<<<(nBlocks + B2Z_LIT_BLOCKS - 1u) / B2Z_LIT_BLOCKS, B2Z_LIT_BLOCKS * 4u, B2Z_LIT_BLOCKS * 4096u, stLit>>>(src, srcSize, blocks, nBlocks, lits, hufTabs, litJobs); }
-    { uint32_t grid = (nBlocks + D1_WARPS(1) - 1) / D1_WARPS(1); if (grid > 148u * 16u) grid = 148u * 16u;
+    { uint32_t grid = (nBlocks + D1_WARPS(1) - 1) / D1_WARPS(1); if (grid > cap) grid = cap;
       zstd_dec_entropy_kernel<1><<<grid, D1_WARPS(1) * 32, 0, st>>>(src, srcSize, blocks, nBlocks, lits, hufTabs, litJobs, seqTabs, seqJobs);
       zstd_dec_seq_streams_kernel<<<(nBlocks + 127u) / 128u, 128, 0, st>>>(src, srcSize, blocks, nBlocks, seqs, seqTabs, seqJobs); }
     if (stLit != st) { cudaEventRecord(evJoin, stLit); cudaStreamWaitEvent(st, evJoin, 0); }
@@ -1235,30 +1237,31 @@ size_t zstd_dec_jump_scratch_bytes(uint64_t total, uint32_t segLog) {         //
     return 256 + ((size_t)seg + 16) * 4 + (size_t)((seg + 127) >> 7) + 64;
 }
 void launch_zstd_dec_jump(const uint8_t* src, DecFrame* frames, uint32_t nFrames, DecBlock* blocks, uint32_t nBlocks, const uint8_t* lits, const uint64_t* seqs,
-                          uint8_t* dst, uint64_t total, uint32_t segLog, DecCounts* counts, void* scratch, cudaStream_t st) {
+                          uint8_t* dst, uint64_t total, uint32_t segLog, DecCounts* counts, void* scratch, uint32_t smCount, cudaStream_t st) {
     if (!nFrames || !nBlocks || !total) return;
     const uint64_t seg = 1ull << segLog, segWords = total < seg ? total : seg;
     uint32_t* flags = (uint32_t*)scratch; uint32_t* ptr = (uint32_t*)((uint8_t*)scratch + 256);
     uint8_t* tileDone = (uint8_t*)(ptr + segWords + 16);
+    const uint32_t cap = smCount * 16u;
     for (uint64_t S = 0; S < total; S += seg) {                        // segments in order: what lies before a segment is complete
         const uint64_t E = S + seg < total ? S + seg : total;
         cudaMemsetAsync(flags, 0, (B2Z_DEC_JUMP_ROUNDS + 1u) * 4u, st);
         cudaMemsetAsync(tileDone, 0, (size_t)((E - S + 127) >> 7), st);
-        { const uint32_t want = (nBlocks + 3u) / 4u, grid = want < 148u * 16u ? want : 148u * 16u;
+        { const uint32_t want = (nBlocks + 3u) / 4u, grid = want < cap ? want : cap;
           zstd_dec_jump_build_kernel<<<grid, 128, 0, st>>>(src, frames, blocks, nBlocks, lits, seqs, dst, counts, ptr, S, E); }
         const uint64_t groups = (E - S + 3u) >> 2;
-        const uint32_t grid = (uint32_t)((groups + 255u) / 256u < 148u * 16u ? (groups + 255u) / 256u : 148u * 16u);
+        const uint32_t grid = (uint32_t)((groups + 255u) / 256u < cap ? (groups + 255u) / 256u : cap);
         for (uint32_t r = 0; r < B2Z_DEC_JUMP_ROUNDS; r++) zstd_dec_jump_round_kernel<false><<<grid, 256, 0, st>>>(frames, nFrames, S, E, ptr, flags, tileDone, r, dst, counts);
         zstd_dec_jump_round_kernel<true><<<grid, 256, 0, st>>>(frames, nFrames, S, E, ptr, flags, tileDone, 0, dst, counts);
     }
 }
 size_t zstd_dec_unit_state_bytes(uint32_t nFrames, uint32_t nBlocks) { return ((size_t)nBlocks / B2Z_DEC_UNIT_BLOCKS + nFrames + 2u) * 4u; }
 void launch_zstd_dec_exec(const uint8_t* src, DecFrame* frames, uint32_t nFrames, DecBlock* blocks, uint32_t nBlocks, const uint8_t* lits, const uint64_t* seqs,
-                          uint8_t* dst, DecCounts* counts, uint32_t* unitState, cudaStream_t st) {
+                          uint8_t* dst, DecCounts* counts, uint32_t* unitState, uint32_t smCount, cudaStream_t st) {
     if (!nFrames) return;
     cudaMemsetAsync(unitState, 0, zstd_dec_unit_state_bytes(nFrames, nBlocks), st);
     const uint32_t maxUnits = nBlocks / B2Z_DEC_UNIT_BLOCKS + nFrames;          // every frame rounds up once
-    const uint32_t grid = maxUnits < 148u * 32u ? maxUnits : 148u * 32u;        // resident warps; the others' units are taken by whoever finishes
+    const uint32_t resident = smCount * 32u, grid = maxUnits < resident ? maxUnits : resident;        // resident warps; the others' units are taken by whoever finishes
     zstd_dec_exec_kernel<<<grid, 32, 0, st>>>(src, frames, nFrames, blocks, lits, seqs, dst, counts, unitState);
 }
 #endif

@@ -170,7 +170,7 @@ static int dec_impl(b200z_ctx* ctx, const void* d_src, size_t srcSize, void* d_d
     if (aLits.reserve((size_t)hc.nSlots * 131072ull + 64) || aSeqs.reserve((size_t)hc.nSlots * B2Z_DEC_MAXSEQ * 8ull + 64) ||
         ctx->decScratch[5].reserve(zstd_dec_entropy_scratch_bytes(hc.nBlocks) + zstd_dec_unit_state_bytes(hc.nFrames, hc.nBlocks) + 64))
         return fail(ctx, B200Z_E_MEMORY, "decoder scratch allocation failed (input too large for one pass)%s");
-    launch_zstd_dec_entropy((const uint8_t*)d_src, srcSize, blocks, hc.nBlocks, (uint8_t*)aLits.p, (uint64_t*)aSeqs.p, ctx->decScratch[5].p, st, st, ctx->ev[4], ctx->ev[5]);
+    launch_zstd_dec_entropy((const uint8_t*)d_src, srcSize, blocks, hc.nBlocks, (uint8_t*)aLits.p, (uint64_t*)aSeqs.p, ctx->decScratch[5].p, ctx->smCount, st, st, ctx->ev[4], ctx->ev[5]);
     CU(cudaGetLastError());
     CU(cudaEventRecord(ctx->ev[1], st));
     // stage J (zstd_dec.cu): frames whose units would form one chain -- what the reference's encoder writes -- are resolved by pointer
@@ -188,7 +188,7 @@ static int dec_impl(b200z_ctx* ctx, const void* d_src, size_t srcSize, void* d_d
             const uint32_t segLog = ctx->decJumpSegLog;
             if (aPtr.reserve(zstd_dec_jump_scratch_bytes(hj.total, segLog))) return fail(ctx, B200Z_E_MEMORY, "decoder scratch allocation failed (stage J pointers)%s");
             launch_zstd_dec_jump((const uint8_t*)d_src, frames, hc.nFrames, blocks, hc.nBlocks, (const uint8_t*)aLits.p, (const uint64_t*)aSeqs.p,
-                                 (uint8_t*)d_dst, hj.total, segLog, counts, aPtr.p, st);
+                                 (uint8_t*)d_dst, hj.total, segLog, counts, aPtr.p, ctx->smCount, st);
             CU(cudaGetLastError());
             ctx->stat[B200Z_S_KERNEL_LAUNCHES] += (2 + B2Z_DEC_JUMP_ROUNDS) * ((hj.total + (1ull << segLog) - 1) >> segLog);
             ctx->stat[B200Z_S_DEC_JUMP_FRAMES] += hj.c.nJump;
@@ -196,7 +196,7 @@ static int dec_impl(b200z_ctx* ctx, const void* d_src, size_t srcSize, void* d_d
     }
     uint32_t* unitState = (uint32_t*)((uint8_t*)ctx->decScratch[5].p + ((zstd_dec_entropy_scratch_bytes(hc.nBlocks) + 15u) & ~(size_t)15u));   // behind D1's scratch
     launch_zstd_dec_exec((const uint8_t*)d_src, frames, hc.nFrames, blocks, hc.nBlocks, (const uint8_t*)aLits.p, (const uint64_t*)aSeqs.p,
-                         (uint8_t*)d_dst, counts, unitState, st);
+                         (uint8_t*)d_dst, counts, unitState, ctx->smCount, st);
     CU(cudaGetLastError());
     launch_zstd_dec_verify((const uint8_t*)d_src, frames, hc.nFrames, (const uint8_t*)d_dst, counts, st);
     CU(cudaGetLastError());

@@ -1,4 +1,4 @@
-// zstd_enc_dp.cu -- stage G of the block-parallel Zstandard encoder (sm_100a): the parse.
+// zstd_enc_dp.cu -- stage G of the block-parallel Zstandard encoder (sm_90a): the parse.
 //
 // One WARP owns one 128 KiB block, one LANE one 4 KiB segment of it (B2Z_SEG): 32 768 blocks x 32 lanes per 4 GiB, so the
 // strictly sequential part of the parse -- a minimum-price path -- runs as a million independent chains.  Per block:

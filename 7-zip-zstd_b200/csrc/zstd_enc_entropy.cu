@@ -1,4 +1,4 @@
-// zstd_enc_entropy.cu -- stage E of the block-parallel Zstandard encoder (sm_100a).
+// zstd_enc_entropy.cu -- stage E of the block-parallel Zstandard encoder (sm_90a).
 //
 // One WARP compresses one 128 KiB block from stage M's output (final sequences + literal
 // bytes) into a complete zstd block (3-byte header + literals section + sequences section)
@@ -627,10 +627,11 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
 #ifndef B2Z_CUEMU
 void launch_zstd_enc_entropy(const uint8_t* src, uint64_t srcSize, const EncGeom& g,
                              const uint64_t* seqs, const uint32_t* nseq, const uint8_t* lits, const uint32_t* nlit,
-                             uint8_t* slots, uint32_t* slotSize, uint32_t nBlocks, cudaStream_t st) {
+                             uint8_t* slots, uint32_t* slotSize, uint32_t nBlocks, uint32_t smCount, cudaStream_t st) {
     if (!nBlocks) return;
     uint32_t grid = (nBlocks + B2Z_ENT_WARPS - 1) / B2Z_ENT_WARPS;
-    if (grid > 148u * 16u) grid = 148u * 16u;
+    const uint32_t cap = smCount * 16u;
+    if (grid > cap) grid = cap;
     zstd_enc_entropy_kernel<<<grid, B2Z_ENT_WARPS * 32, 0, st>>>(src, srcSize, g, seqs, nseq, lits, nlit, slots, slotSize, nBlocks);
 }
 #endif

@@ -1,4 +1,4 @@
-// zstd_enc_find.cu -- stage F of the block-parallel Zstandard encoder (sm_100a): the match finder.
+// zstd_enc_find.cu -- stage F of the block-parallel Zstandard encoder (sm_90a): the match finder.
 //
 // One CTA owns one independent frame (2^frameLog input bytes) and keeps BOTH hash tables of the finder in its shared
 // memory (long: 2^hashLogL entries indexed by the 8-byte hash, short: 2^hashLogS entries indexed by the 5-byte hash;

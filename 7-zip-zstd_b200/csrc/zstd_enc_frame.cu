@@ -1,4 +1,4 @@
-// zstd_enc_frame.cu -- frame assembly for the block-parallel Zstandard encoder (sm_100a).
+// zstd_enc_frame.cu -- frame assembly for the block-parallel Zstandard encoder (sm_90a).
 //
 // Stage E leaves every compressed block (3-byte header + body) in a fixed-stride slot.  Here
 //   1. one CTA scans the slot sizes (plus per-frame header/trailer bytes) into output offsets;

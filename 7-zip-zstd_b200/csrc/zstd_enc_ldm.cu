@@ -1,4 +1,4 @@
-// zstd_enc_ldm.cu -- stage L of the Zstandard encoder's long mode (sm_100a): matches up to a window of 128 MiB back, in frames of 8 windows.
+// zstd_enc_ldm.cu -- stage L of the Zstandard encoder's long mode (sm_90a): matches up to a window of 128 MiB back, in frames of 8 windows.
 //
 // The long mode (B200Z_P_LONG; the reference's long=N -> ZSTD_c_enableLongDistanceMatching + windowLog N, ZstdEncoder.cpp:128-146,
 // 322-331, algorithm zstd_ldm.c:333-470) keeps stage F as it is -- one CTA per REGION of 2^regionLog bytes, tables in shared

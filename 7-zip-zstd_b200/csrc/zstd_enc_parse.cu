@@ -1,4 +1,4 @@
-// zstd_enc_parse.cu -- stage Z: the price-based parse of the block-parallel Zstandard encoder (flag B2Z_FLAG_ZSTD_OPT) for sm_100a.
+// zstd_enc_parse.cu -- stage Z: the price-based parse of the block-parallel Zstandard encoder (flag B2Z_FLAG_ZSTD_OPT) for sm_90a.
 //
 // Replaces stage M for the high levels: stage C (lzma2_parse.cu: nearest-occurrence candidates by 3/4/6/8-byte keys, shared with
 // method 21) runs first, then this kernel, one WARP per 128 KiB BLOCK -- blocks never share repcode history or entropy tables in

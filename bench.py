@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 zstd hot path (BASELINE.json configs[1]).
+"""bench.py -- headline benchmark of the zstd hot path on one H100 (BASELINE.json configs[1]).
 
 One "step" = one pass of the hot path over one batch of synthetic input: zstd level-3 encode of
 the rank's corpus shard followed by decode of the produced frames (round trip verified on the
 device, outside the timed region).  Metric: MB/s of uncompressed data through encode+decode,
 MB = 1e6 bytes:   value = units / (t_enc + t_dec).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--size-mib M] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--size-mib M] [--impl ours|reference] [--dump-outputs DIR]
   torchrun --nproc-per-node N bench.py --gpus N ...        (one rank per GPU, weak scaling)
 
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for the definitions.
@@ -35,8 +35,8 @@ def parse_args():
     ap.add_argument("--no-files-extra", action="store_true", help="skip extra.many_files_7z (BASELINE configs[4]: 100 000 files of 64 KiB -> one non-solid .7z, one GPU pass)")
     ap.add_argument("--no-lzma2-extra", action="store_true", help="skip extra.lzma2 (BASELINE configs[3] measured beside the zstd headline: method 21 as -m0=flzma2 -mx5 selects it)")
     ap.add_argument("--no-refstreams-extra", action="store_true", help="skip extra.reference_streams (reference-written single-frame zstd and stock LZMA2 streams through the engine's decoders)")
-    ap.add_argument("--no-long-extra", action="store_true", help="skip extra.long_range (BASELINE configs[2]: 8 GiB of text with far copies, long=27)")
-    ap.add_argument("--long-mib", type=int, default=8192, help="extra.long_range: MiB of G3 input (configs[2]: 8 GiB)")
+    ap.add_argument("--no-long-extra", action="store_true", help="skip extra.long_range (BASELINE configs[2]: text with far copies, long=27)")
+    ap.add_argument("--long-mib", type=int, default=4096, help="extra.long_range: MiB of G3 input (8 GiB does not fit an 80 GB H100)")
     ap.add_argument("--codec", default="zstd", choices=["zstd", "lzma2"],
                     help="zstd: method 4F71101 level 3 (the headline, BASELINE configs[1]); lzma2: method 21 (configs[3])")
     ap.add_argument("--level", type=int, default=3, help="--codec zstd: B200Z_P_LEVEL (1-7 stage M, the measured headline; 8-22 the price-based stage C + stage Z)")
@@ -49,7 +49,28 @@ def parse_args():
                     help="no torchrun: ONE process, one context over --gpus N devices (b200z_create_multi), the whole --size-mib input through the host-pointer calls "
                          "(strong scaling: what one ICompressCoder::Code() call gets from the box)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy")
     return ap.parse_args()
+
+
+DUMP_SAMPLES = 4_000_000        # bytes sampled from each output: 2 x 16 MB of float32
+
+
+def dump_outputs(out_dir, d_comp, csize, d_back, extra_sizes=()):
+    """The timed path's last step as .npy files: a fixed seeded sample of the compressed stream and of the restored bytes (float32),
+    and the stream sizes plus whole-output CRC32s (float64, exact) so that a difference outside the samples still shows."""
+    import zlib
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.RandomState(20240601)
+    for name, d, n in (("compressed", d_comp, csize), ("decompressed", d_back, d_back.numel())):
+        idx = np.sort((rng.random_sample(min(DUMP_SAMPLES, n)) * n).astype(np.int64))
+        np.save(os.path.join(out_dir, f"{name}.npy"), d[torch.from_numpy(idx).to(d.device)].cpu().numpy().astype(np.float32))
+    comp, back = d_comp[:csize].cpu().numpy(), d_back.cpu().numpy()
+    np.save(os.path.join(out_dir, "sizes.npy"), np.array([csize, d_back.numel(), *extra_sizes], dtype=np.float64))
+    np.save(os.path.join(out_dir, "crc32.npy"), np.array([zlib.crc32(comp), zlib.crc32(back)], dtype=np.float64))
 
 
 # ---------------------------------------------------------------- clocks sampler (nvidia-smi)
@@ -445,17 +466,21 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
-    codec = pkg.Codec(local)
     if lz and not a.frame_log:
         a.frame_log = 23                                            # fl2_compress.c:80: level 5 = 8 MiB dictionary; a frame = one dictionary-reset block
-    if a.frame_log:
-        codec.set("frame_log", a.frame_log); codec.set("window_log", a.frame_log)
-    if not lz and a.level != 3:
-        codec.set("level", a.level)
-    if lz and a.lzma2_slice_log >= 0:
-        codec.set("lzma2_slice_log", a.lzma2_slice_log)
-    if lz and a.lzma2_parse:
-        codec.set("lzma2_parse", 1)
+
+    def make_codec():
+        codec = pkg.Codec(local)
+        if a.frame_log:
+            codec.set("frame_log", a.frame_log); codec.set("window_log", a.frame_log)
+        if not lz and a.level != 3:
+            codec.set("level", a.level)
+        if lz and a.lzma2_slice_log >= 0:
+            codec.set("lzma2_slice_log", a.lzma2_slice_log)
+        if lz and a.lzma2_parse:
+            codec.set("lzma2_parse", 1)
+        return codec
+    codec = make_codec()
     # ---- corpus shard: rank r owns bytes [r*unit, (r+1)*unit) of the seeded G2 stream (weak scaling)
     host_in = torch.empty(unit_bytes, dtype=torch.uint8).pin_memory()
     pkg.corpus.g2_into(host_in.data_ptr(), unit_bytes, offset=rank * unit_bytes, threads=max(1, (os.cpu_count() or 8) // max(1, world)))
@@ -464,11 +489,14 @@ def main():
     d_comp = torch.empty(bound, dtype=torch.uint8, device="cuda")
     d_back = torch.empty(unit_bytes, dtype=torch.uint8, device="cuda")
 
+    lzma2_prop = [0]
+
     def step_device():
         if lz:
             t0 = time.perf_counter(); c, prop = codec.lzma2_compress_device(d_in.data_ptr(), unit_bytes, d_comp.data_ptr(), bound); t1 = time.perf_counter()
             n = codec.lzma2_decompress_device(d_comp.data_ptr(), c, prop, d_back.data_ptr(), unit_bytes); t2 = time.perf_counter()
             assert n == unit_bytes
+            lzma2_prop[0] = prop
             return c, t1 - t0, t2 - t1
         t0 = time.perf_counter(); c = codec.compress_device(d_in.data_ptr(), unit_bytes, d_comp.data_ptr(), bound); t1 = time.perf_counter()
         n = codec.decompress_device(d_comp.data_ptr(), c, d_back.data_ptr(), unit_bytes); t2 = time.perf_counter()
@@ -476,18 +504,20 @@ def main():
         return c, t1 - t0, t2 - t1
 
     for _ in range(a.warmup):
-        csize, _, _ = step_device()
-    assert torch.equal(d_back, d_in), "round trip mismatch"                      # bit-exact round trip (outside the timed region)
-    ratio = unit_bytes / csize
+        step_device()
 
     sampler = ClockSampler(local); sampler.start()
     codec.reset_stats()
     barrier(); T0 = time.perf_counter()
     t_enc = t_dec = 0.0
     for _ in range(a.steps):
-        _, te, td = step_device(); t_enc += te; t_dec += td
+        csize, te, td = step_device(); t_enc += te; t_dec += td
     barrier(); T1 = time.perf_counter()
     clocks = sampler.stop(T0, T1)
+    assert torch.equal(d_back, d_in), "round trip mismatch"                      # bit-exact round trip of the last timed step (outside the timed region)
+    ratio = unit_bytes / csize
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, d_comp, csize, d_back, (lzma2_prop[0],) if lz else ())
     elapsed = T1 - T0
     stats = {k: codec.stat(v) for k, v in dict(match_ms=1, entropy_ms=2, assemble_ms=3, dec_prepass_ms=9, dec_entropy_ms=4, dec_exec_ms=5, launches=6, parse_ms=10).items()}
     if dist:
@@ -542,12 +572,7 @@ def main():
         return
     # ---- roofline of the dominant kernel (stage F, zstd_enc_find_kernel): algorithmic bytes per launch
     #      = U * (1 + 1/ratio)  (SURVEY.md 8(d): encode reads the input once, writes the compressed stream once)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = peaks.get("hbm_gbs", 6650.0); peak_src = "measured" if "hbm_gbs" in peaks else "fallback"
+    peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3)"
     # LZMA2: the dominant kernel is stage R (lzma2_enc_range_kernel: one serial range-coder chain per 1 MiB block)
     #        with the price-based parse it is stage P (lzma2_parse_kernel: one dynamic-programme chain per slice)
     zparse = (not lz) and a.level >= 8
@@ -555,12 +580,6 @@ def main():
     match_ms = ((stats["parse_ms"] if a.lzma2_parse else stats["entropy_ms"]) if lz else (stats["parse_ms"] if zparse else stats["match_ms"])) / a.steps
     algo_bytes = unit_bytes * (1.0 + 1.0 / ratio)
     achieved = algo_bytes / 1e9 / (match_ms / 1e3) if match_ms > 0 else 0.0
-    traffic = None
-    try:
-        if not (lz and a.lzma2_parse) and not zparse:               # no ncu capture of stage P / stage Z yet
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "r1_lzma2_range_traffic.json" if lz else "r2_find_traffic.json")))["dram_bytes_per_input_byte"] * unit_bytes
-    except Exception:
-        pass
     line = {
         "metric": metric_name, "value": value, "unit": "MB/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
         "ms_per_step": 1e3 * elapsed / a.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
@@ -570,7 +589,7 @@ def main():
                    "ratio": ratio, "enc_MBps": units_mb / t_enc, "dec_MBps": units_mb / t_dec,
                    "kernel_ms_per_step": {k: v / a.steps for k, v in stats.items() if k != "launches"}},
         "roofline": {"bound": "hbm", "kernel": dom_kernel, "achieved": achieved, "peak": peak, "peak_source": peak_src, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": traffic, "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": match_ms},
+                     "frac": achieved / peak, "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": match_ms},
         "clocks": clocks, "gpu_launches": int(stats["launches"]), "e2e": e2e,
     }
     if multi:
@@ -580,6 +599,7 @@ def main():
         # 8 MiB dictionary-reset blocks), the same 4 GiB resident in HBM, one timed pass after a small warm-up; the reference's FL2 level 5
         # on a bounded sample of the same text beside it
         del d_comp, d_back
+        codec.close()                                               # 80 GB hold one codec's scratch at a time, not two
         torch.cuda.empty_cache()
         lc = pkg.Codec(local, lzma2_parse=1, frame_log=23, window_log=23)
         lb = lc.lzma2_compress_bound(unit_bytes)
@@ -605,6 +625,7 @@ def main():
         lc.close()
         del l_comp, l_back
         torch.cuda.empty_cache()
+        codec = make_codec()
     if not lz and world == 1 and not a.no_files_extra:
         try:
             line.setdefault("extra", {})["many_files_7z"] = many_files_7z(pkg, codec, cpu=not a.no_cpu_baseline)
@@ -613,6 +634,7 @@ def main():
     if not lz and world == 1 and not a.no_long_extra:
         try:
             del d_in
+            codec.close()                                           # its scratch and the long mode's do not fit 80 GB together
             torch.cuda.empty_cache()
             line.setdefault("extra", {})["long_range"] = long_range(pkg, local, a.long_mib, cpu=not a.no_cpu_baseline)
         except Exception as e:

@@ -1,4 +1,4 @@
-/* b200z.h -- C ABI of libb200z.so: the B200 block-parallel codec engine behind 7-Zip's
+/* b200z.h -- C ABI of libb200z.so: the H100 block-parallel codec engine behind 7-Zip's
  * ZSTD (method 4F71101) and LZMA2/FLZMA2 (method 21) coders.
  *
  * This is the drop-in boundary: plain pointers and sizes, no C++/torch types.  The host-side

@@ -1,4 +1,4 @@
-/* lzma2_enc_oracle.c -- sequential statement of the B200 LZMA2 encoder (7-Zip method 21).
+/* lzma2_enc_oracle.c -- sequential statement of the GPU LZMA2 encoder (7-Zip method 21).
  *
  * TEST INFRASTRUCTURE ONLY (see oracle.h).  The encoder's byte stream is ours (the reference pins no encoder bytes,
  * SURVEY.md 8c); what is pinned: the reference decoder (C/Lzma2Dec.c via oracle/_ref), liblzma and the oracle decoder all

@@ -1,4 +1,4 @@
-/* lzma2_opt_oracle.c -- sequential statement of the price-based parse of the B200 LZMA2 encoder (method 21, flag B2Z_FLAG_LZ2_OPT).
+/* lzma2_opt_oracle.c -- sequential statement of the price-based parse of the GPU LZMA2 encoder (method 21, flag B2Z_FLAG_LZ2_OPT).
  *
  * TEST INFRASTRUCTURE ONLY (see oracle.h).  States what csrc/lzma2_parse.cu computes:
  *

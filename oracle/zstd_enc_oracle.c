@@ -1,4 +1,4 @@
-/* zstd_enc_oracle.c -- plain-C restatement of the B200 block-parallel Zstandard encoder.
+/* zstd_enc_oracle.c -- plain-C restatement of the GPU block-parallel Zstandard encoder.
  *
  * TEST INFRASTRUCTURE ONLY (see oracle.h).  This is the single-threaded statement of the
  * algorithm that 7-zip-zstd_b200/csrc/zstd_enc_*.cu implements with one CTA per frame

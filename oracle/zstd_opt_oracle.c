@@ -1,4 +1,4 @@
-/* zstd_opt_oracle.c -- sequential statement of the price-based parse of the B200 Zstandard encoder (stage Z; flag B2Z_FLAG_ZSTD_OPT).
+/* zstd_opt_oracle.c -- sequential statement of the price-based parse of the GPU Zstandard encoder (stage Z; flag B2Z_FLAG_ZSTD_OPT).
  *
  * TEST INFRASTRUCTURE ONLY (see oracle.h).  States what csrc/zstd_enc_parse.cu computes for one frame: per 128 KiB block, the
  * sequences and literal bytes stage E codes (same arrays as stage M, b2zo_zstd_find_sequences).

@@ -141,6 +141,16 @@ def ref_compress(data, level=3, checksum=0, **kw) -> bytes:
     return out[:r].tobytes()
 
 
+def ref_zstd_size(data, key) -> int:
+    """bytes the reference's level 3 writes for `data`: computed where oracle/_ref is built (and checked against the stored figure),
+    the stored figure of tests/golden/ref_zstd_sizes.json elsewhere"""
+    import json
+    stored = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_zstd_sizes.json")))[key]
+    if ref_available():
+        assert len(ref_compress(data, 3)) == stored, key
+    return stored
+
+
 def ref_decompress(comp, n) -> bytes:
     Z = ref()
     dst = np.empty(n + 1, dtype=np.uint8); src = _np(comp)

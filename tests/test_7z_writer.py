@@ -59,6 +59,9 @@ def _check_archive(arc_bytes, files, names, tmp_path, shown="ZSTD:v1.5,l3"):
         assert (outdir / n).read_bytes() == f, n
 
 
+VERIFIED = os.path.join(ROOT, "tests", "golden", "ref_7zz_verified.json")     # SHA-256 of archives the stock 7zz tested, listed and extracted
+
+
 def test_container_writer_on_oracle_frames(pkg, tmp_path):
     files, names = _files(pkg, 60)
     L = pkg.load_library()
@@ -74,7 +77,11 @@ def test_container_writer_on_oracle_frames(pkg, tmp_path):
                                   out.ctypes.data, cap, ctypes.byref(n))
     assert rc == 0
     assert out[:6].tobytes() == b"7z\xbc\xaf\x27\x1c"
-    _check_archive(out[:n.value].tobytes(), files, names, tmp_path)
+    import hashlib, json
+    digest = hashlib.sha256(out[:n.value].tobytes()).hexdigest()
+    assert digest == json.load(open(VERIFIED))["container_writer_on_oracle_frames"]   # the bytes the reference accepted
+    if os.path.exists(STOCK):                                                    # and the reference itself where it is built
+        _check_archive(out[:n.value].tobytes(), files, names, tmp_path)
     # too small a destination is refused, nothing is written past it
     assert L.b200z_7z_build_archive(blob.ctypes.data, pack.ctypes.data, unpack.ctypes.data, crcs.ctypes.data, arr, None, len(files), 3, out.ctypes.data, 100, ctypes.byref(n)) == -4
 

@@ -74,10 +74,8 @@ def test_params_and_hints(pkg, inputs):
 
 def test_ratio_vs_reference_level3(pkg, codec):
     """ratio within 1 % of the reference's level 3 on the BASELINE cfg2 text shape (16 MiB sample)."""
-    if not helpers.ref_available():
-        pytest.skip("oracle/_ref not built")
     data = pkg.corpus.g2(16 << 20).tobytes()
-    ours = len(codec.compress(data)); ref = len(helpers.ref_compress(data, 3))
+    ours = len(codec.compress(data)); ref = helpers.ref_zstd_size(data, "g2_16MiB_level3")
     assert ours <= ref * 1.01, (ours, ref)
 
 

@@ -1,8 +1,8 @@
 """Longer differential run of stage J in the host emulation (test infrastructure): reference-written and own frames, intact and damaged, through
 the jump kernels forced on every frame with segment sizes of 64 KiB / 128 KiB / 1 GiB; the oracle decoder's verdict and bytes are the bar.
 usage: python tools/fuzz_stage_j.py <seed> <seconds>"""
-import sys, ctypes, random, time
-sys.path[:0]=['/root/repo','/root/repo/tests']
+import os, sys, ctypes, random, time
+_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path[:0] = [_ROOT, os.path.join(_ROOT, "tests")]
 import numpy as np
 import __graft_entry__ as ge, helpers as H
 pkg=ge.load_package(); E=H.cuemu_library()
