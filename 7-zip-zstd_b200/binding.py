@@ -140,13 +140,18 @@ class Codec:
 
     _PARAMS = dict(level=P_LEVEL, frame_log=P_FRAMELOG, hash_log_l=P_HASHLOG_L, hash_log_s=P_HASHLOG_S,
                    window_log=P_WINDOWLOG, flags=P_FLAGS, batch_log=P_BATCH_LOG, host_batch_log=8, chunk_log=9, lzma2_model=10, lzma2_slice_log=11, lzma2_parse=12, zstd_parse=13, long=14, region_log=15, dec_jump=16, dec_jump_seg_log=17)
+    # the LZMA2 encoder's literal / position context bits (B200Z_P_LZMA2_LC/LP/PB), kept beside _PARAMS, whose names tests pin
+    _LZMA2_CONTEXT_PARAMS = dict(lzma2_lc=18, lzma2_lp=19, lzma2_pb=20)
+
+    def _param_id(self, name):
+        return self._PARAMS[name] if name in self._PARAMS else self._LZMA2_CONTEXT_PARAMS[name]
 
     def set(self, name, value):
-        self._check(self.L.b200z_set_param(self.h, self._PARAMS[name], int(value)))
+        self._check(self.L.b200z_set_param(self.h, self._param_id(name), int(value)))
 
     def get(self, name):
         v = ctypes.c_int64()
-        self._check(self.L.b200z_get_param(self.h, self._PARAMS[name], ctypes.byref(v)))
+        self._check(self.L.b200z_get_param(self.h, self._param_id(name), ctypes.byref(v)))
         return v.value
 
     def stat(self, s):

@@ -22,4 +22,5 @@ gcc -O2 -shared -fPIC -pthread -o corpus/libb200z_corpus.so corpus/g2gen.c
 # 7-Zip codec module (ICompressCoder classes + CodecExports) and its C++ test driver
 g++ -std=c++17 -O2 -fPIC -shared -Wall -Wno-misleading-indentation codec/ZstdCoders.cpp codec/Lzma2Coders.cpp -I../include -L. -lb200z -Wl,-rpath,'$ORIGIN' -o libb200z_7z.so
 g++ -std=c++17 -O2 ../tests/cpp/coder_roundtrip.cpp -ldl -o build/coder_roundtrip
+g++ -std=c++17 -O2 ../tests/cpp/coder_props.cpp -ldl -o build/coder_props
 echo "built $(pwd)/libb200z.so"

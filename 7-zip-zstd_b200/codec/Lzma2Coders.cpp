@@ -21,6 +21,7 @@ class CLzma2Encoder final : public ICompressCoder, public ICompressSetCoderPrope
     const bool fast_;
     int frameLog_ = 20;                                        // 1 MiB blocks: thousands of independent blocks per GiB
     int level_ = -1, algo_ = -1;                               // kLevel / kAlgorithm as given (-1: not given)
+    int lc_ = -1, lp_ = -1, pb_ = -1;                          // kLitContextBits / kLitPosBits / kPosStateBits (-1: the engine's 2 / 0 / 2)
     PinnedBuf in_, out_;
 public:
     UInt64 processedIn = 0, processedOut = 0;
@@ -39,6 +40,7 @@ public:
 
     HRESULT SetCoderProperties(const PROPID* ids, const PROPVARIANT* pv, UInt32 n) override {
         uint64_t blockSize = 0, dictSize = 0;
+        int lc = -1, lp = -1, pb = -1;                         // every call starts from the defaults, as Lzma2EncProps_Init does
         for (UInt32 i = 0; i < n; i++) {
             const PROPVARIANT& p = pv[i];
             switch (ids[i]) {
@@ -51,13 +53,19 @@ public:
             case NCoderPropID::kAlgorithm: if (p.vt != VT_UI4) return E_INVALIDARG; if (fast_ && p.ulVal > 3) return E_INVALIDARG;      // Lzma2Encoder.cpp:197-199
                 algo_ = (int)p.ulVal; break;
             case NCoderPropID::kLevel: if (p.vt != VT_UI4) return E_INVALIDARG; level_ = (int)p.ulVal; break;
-            case NCoderPropID::kLitContextBits: case NCoderPropID::kLitPosBits: case NCoderPropID::kPosStateBits:
+            // LzmaEnc_SetProps (LzmaEnc.c:541): lc <= 8, lp <= 4, pb <= 4; fast-lzma2 (fl2_compress.c:720-737): lc <= 4
+            case NCoderPropID::kLitContextBits: if (p.vt != VT_UI4 || p.ulVal > (fast_ ? 4u : 8u)) return E_INVALIDARG; lc = (int)p.ulVal; break;
+            case NCoderPropID::kLitPosBits: if (p.vt != VT_UI4 || p.ulVal > 4) return E_INVALIDARG; lp = (int)p.ulVal; break;
+            case NCoderPropID::kPosStateBits: if (p.vt != VT_UI4 || p.ulVal > 4) return E_INVALIDARG; pb = (int)p.ulVal; break;
             case NCoderPropID::kNumFastBytes: case NCoderPropID::kMatchFinderCycles:
-                if (p.vt != VT_UI4) return E_INVALIDARG;      // accepted; the GPU coder runs lc2 lp0 pb2 and its own finder
+                if (p.vt != VT_UI4) return E_INVALIDARG;      // accepted; the GPU coder runs its own finder
                 break;
             default: break;                                    // kMatchFinder, kEndMarker, kReduceSize, kAffinity ...: accepted
             }
         }
+        // LZMA2 keeps lc + lp <= 4 (Lzma2Enc_SetProps, Lzma2Enc.c:471; fast-lzma2 lclpMax_exceeded); a property not given is the engine's
+        if ((lc < 0 ? 2 : lc) + (lp < 0 ? 0 : lp) > 4) return E_INVALIDARG;
+        lc_ = lc; lp_ = lp; pb_ = pb;
         // independent block = dictionary = frame: the explicit block size wins, else the dictionary size, else 1 MiB
         const uint64_t want = (blockSize && blockSize != ~0ull) ? blockSize : dictSize;
         if (want) { int fl = log2_floor(want); frameLog_ = fl < 17 ? 17 : (fl > 24 ? 24 : fl); }
@@ -83,6 +91,9 @@ public:
         b200z_set_param(ctx, B200Z_P_FRAMELOG, frameLog_);
         b200z_set_param(ctx, B200Z_P_WINDOWLOG, frameLog_);
         b200z_set_param(ctx, B200Z_P_LZMA2_PARSE, price_parse());
+        b200z_set_param(ctx, B200Z_P_LZMA2_LC, lc_ < 0 ? 2 : lc_);
+        b200z_set_param(ctx, B200Z_P_LZMA2_LP, lp_ < 0 ? 0 : lp_);
+        b200z_set_param(ctx, B200Z_P_LZMA2_PB, pb_ < 0 ? 2 : pb_);
         const size_t batch = (size_t)1 << 30;                  // 1 GiB of input per GPU pass (about a thousand blocks)
         if (!in_.reserve(batch) || !out_.reserve(b200z_lzma2_compress_bound(ctx, batch))) return E_OUTOFMEMORY;
         for (;;) {

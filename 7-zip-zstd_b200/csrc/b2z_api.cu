@@ -149,6 +149,10 @@ static int set_param_one(b200z_ctx* ctx, int param, int64_t v) {
                             ctx->geom.regionLog = (uint32_t)v; return 0;
     case B200Z_P_CHUNKLOG:  if (v < 5 || v > 8) return fail(ctx, B200Z_E_PARAM, "chunkLog out of range%s"); ctx->geom.chunkLog = (uint32_t)v; return 0;
     case B200Z_P_LZMA2_MODEL: if (v < 0 || v > 3) return fail(ctx, B200Z_E_PARAM, "lzma2 model placement out of range%s"); ctx->lz2Mode = (int)v; return 0;
+    // each alone here; lc + lp <= 4 is checked when a compression starts (lz2_check_props), as the values arrive one at a time
+    case B200Z_P_LZMA2_LC: if (v < 0 || v > 4) return fail(ctx, B200Z_E_PARAM, "lzma2 lc out of range (0..4)%s"); ctx->lz2Lc = (uint32_t)v; return 0;
+    case B200Z_P_LZMA2_LP: if (v < 0 || v > 4) return fail(ctx, B200Z_E_PARAM, "lzma2 lp out of range (0..4)%s"); ctx->lz2Lp = (uint32_t)v; return 0;
+    case B200Z_P_LZMA2_PB: if (v < 0 || v > 4) return fail(ctx, B200Z_E_PARAM, "lzma2 pb out of range (0..4)%s"); ctx->lz2Pb = (uint32_t)v; return 0;
     case B200Z_P_DEC_JUMP_SEGLOG: if (v < 16 || v > B2Z_DEC_JUMP_SEGLOG) return fail(ctx, B200Z_E_PARAM, "decoder jump segment log out of range%s"); ctx->decJumpSegLog = (uint32_t)v; return 0;
     case B200Z_P_DEC_JUMP: if (v < 0 || v > 2) return fail(ctx, B200Z_E_PARAM, "decoder jump mode out of range%s"); ctx->decJump = (int)v; return 0;
     case B200Z_P_HOST_BATCH_LOG: if (v < 22 || v > 36) return fail(ctx, B200Z_E_PARAM, "hostBatchLog out of range%s"); ctx->hostBatchLog = (uint32_t)v; return 0;
@@ -173,6 +177,9 @@ int b200z_get_param(b200z_ctx* ctx, int param, int64_t* v) {
     case B200Z_P_DEC_JUMP: *v = ctx->decJump; return 0;
     case B200Z_P_DEC_JUMP_SEGLOG: *v = ctx->decJumpSegLog; return 0;
     case B200Z_P_LZMA2_MODEL: *v = ctx->lz2Mode; return 0;
+    case B200Z_P_LZMA2_LC: *v = ctx->lz2Lc; return 0;
+    case B200Z_P_LZMA2_LP: *v = ctx->lz2Lp; return 0;
+    case B200Z_P_LZMA2_PB: *v = ctx->lz2Pb; return 0;
     case B200Z_P_CHUNKLOG: *v = ctx->geom.chunkLog; return 0;
     case B200Z_P_LONG: *v = ctx->geom.ldmLog ? ctx->geom.windowLog : 0; return 0;
     case B200Z_P_REGIONLOG: *v = ctx->geom.regionLog; return 0;
@@ -218,6 +225,19 @@ static uint32_t cand_warps(const b200z_ctx* ctx, uint64_t nFrames) {
     return (uint32_t)(nFrames < cap ? nFrames : cap);
 }
 
+// LZMA2 encoder context bits -> the flags bits the kernels read (b2z_params.h): none for the defaults, which keep the compile-time
+// instantiations
+static uint32_t lz2_props_flags(const b200z_ctx* ctx) {
+    const uint32_t props = (ctx->lz2Pb * 5u + ctx->lz2Lp) * 9u + ctx->lz2Lc;
+    return props == B2Z_LZ2_PROPS ? 0u : (B2Z_FLAG_LZ2_PROPS | (props << 16));
+}
+int lz2_check_props(b200z_ctx* ctx) {
+    if (ctx->lz2Lc + ctx->lz2Lp > 4u) return fail(ctx, B200Z_E_PARAM, "lzma2: lc + lp must not exceed 4%s");
+    if (ctx->lz2Mode == 3 && ctx->lz2Lc + ctx->lz2Lp > 3u)
+        return fail(ctx, B200Z_E_PARAM, "lzma2: model placement 3 codes lc + lp <= 3 only (its decision queue holds 13-bit probability indices)%s");
+    return 0;
+}
+
 static int enc_reserve(b200z_ctx* ctx, uint64_t batchBytes, int codec = 0) {
     const uint64_t F = 1ull << ctx->geom.frameLog;
     const uint64_t nFrames = (batchBytes + F - 1) / F;
@@ -249,7 +269,8 @@ static int enc_batch(b200z_ctx* ctx, const uint8_t* d_src, uint64_t n, uint8_t* 
                      const uint32_t* ready = nullptr, uint32_t readyShift = 0, int codec = 0) {
     int rc = enc_reserve(ctx, n, codec);
     if (rc) return rc;
-    const EncGeom& g = ctx->geom;
+    EncGeom g = ctx->geom;
+    if (codec == 1) g.flags |= lz2_props_flags(ctx);
     const uint64_t F = 1ull << g.frameLog;
     const uint64_t nFrames = (n + F - 1) / F;
     const uint32_t nBlocks = (uint32_t)((n >> 17) + ((n & (B2Z_BLOCK - 1)) ? 1 : 0));
@@ -292,14 +313,16 @@ static int enc_batch(b200z_ctx* ctx, const uint8_t* d_src, uint64_t n, uint8_t* 
     }
     if (!stageMOnly && codec == 1) {
         // LZMA2: stage R (range coding, one thread per frame) + assembly of the frame slots into one chunk stream
-        constexpr uint32_t LITN = 0x300u << (B2Z_LZ2_LC + B2Z_LZ2_LP);
+        const uint32_t LITN = b2z_lz2_litn(b2z_lz2_props(g.flags));
         uint16_t* spill = nullptr;
         const uint64_t nChains = nFrames * lzma2_enc_slices_per_frame(g);
+        // auto placement: a global literal model is worth allocating above 11 chains per SM, or wherever the shared-memory slots end first
+        const uint32_t spillPerSm = lzma2_enc_smem_chains_per_sm(g.flags) < 11u ? lzma2_enc_smem_chains_per_sm(g.flags) : 11u;
         if (ctx->lz2Mode == 3) {                                    // 32 chains per warp: every chain's whole model in global memory
-            if (ctx->decScratch[5].reserve(lzma2_enc_model_bytes((uint32_t)nChains))) return fail(ctx, B200Z_E_MEMORY, "LZMA2: model allocation failed%s");
+            if (ctx->decScratch[5].reserve(lzma2_enc_model_bytes((uint32_t)nChains, g.flags))) return fail(ctx, B200Z_E_MEMORY, "LZMA2: model allocation failed%s");
             spill = (uint16_t*)ctx->decScratch[5].p;
         } else
-        if (ctx->lz2Mode != 1 && nChains > 11ull * ctx->smCount && ctx->decScratch[5].reserve((size_t)nChains * LITN * 2u) == 0) spill = (uint16_t*)ctx->decScratch[5].p;
+        if (ctx->lz2Mode != 1 && nChains > (uint64_t)spillPerSm * ctx->smCount && ctx->decScratch[5].reserve((size_t)nChains * LITN * 2u) == 0) spill = (uint16_t*)ctx->decScratch[5].p;
         if (ctx->lz2Mode == 2 && !spill) {
             if (ctx->decScratch[5].reserve((size_t)nChains * LITN * 2u)) return fail(ctx, B200Z_E_MEMORY, "LZMA2: model allocation failed%s");
             spill = (uint16_t*)ctx->decScratch[5].p;
@@ -659,6 +682,7 @@ size_t b200z_lzma2_compress_bound(b200z_ctx* ctx, size_t srcSize) {
 
 int b200z_lzma2_compress_device(b200z_ctx* ctx, const void* d_src, size_t srcSize, void* d_dst, size_t dstCap, size_t* dstSize, uint32_t* dictProp) {
     if (!ctx || !dstSize || (!d_src && srcSize) || !d_dst) return B200Z_E_PARAM;
+    { const int prc = lz2_check_props(ctx); if (prc) return prc; }
     if ((uintptr_t)d_src & 15u) return fail(ctx, B200Z_E_PARAM, "device source must be 16-byte aligned%s");
     if (dstCap < b200z_lzma2_compress_bound(ctx, srcSize)) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_lzma2_compress_bound%s");
     if (dictProp) *dictProp = (ctx->geom.frameLog - 12u) * 2u;           // dictionary = frame size (Lzma2Enc_WriteProperties, Lzma2Enc.c:671)
@@ -701,6 +725,7 @@ int b200z_lzma2_enc_stage_cp(b200z_ctx* ctx, const void* d_src, size_t srcSize, 
 // Host-pointer form; one batch: chunked upload overlapped with stage M (as the zstd path), kernels, download.
 int b200z_lzma2_compress_host(b200z_ctx* ctx, const void* src, size_t srcSize, void* dst, size_t dstCap, size_t* dstSize, uint32_t* dictProp) {
     if (!ctx || !dstSize || (!src && srcSize) || !dst) return B200Z_E_PARAM;
+    { const int prc = lz2_check_props(ctx); if (prc) return prc; }
     const size_t bound = b200z_lzma2_compress_bound(ctx, srcSize);
     if (dstCap < bound) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_lzma2_compress_bound%s");
     if (dictProp) *dictProp = (ctx->geom.frameLog - 12u) * 2u;

@@ -40,6 +40,7 @@ struct b200z_ctx {
     uint32_t decJumpSegLog = B2Z_DEC_JUMP_SEGLOG;   // stage J: bytes of output resolved per pass (B200Z_P_DEC_JUMP_SEGLOG; tests use small segments)
     int decJump = 1;                  // Zstandard decoder, stage J (frames resolved by pointer jumping): 0 never, 1 frames whose units form a chain, 2 every frame
     int lz2Mode = 0;                  // LZMA2 decoder literal-model placement: 0 auto, 1 shared memory, 2 global memory
+    uint32_t lz2Lc = B2Z_LZ2_LC, lz2Lp = B2Z_LZ2_LP, lz2Pb = B2Z_LZ2_PB;   // LZMA2 encoder context bits (B200Z_P_LZMA2_LC/LP/PB)
     Arena tables, seqs, nseq, lits, nlit, slots, slotSize, blockOff, frameOff, scalars, dIn, dOut, cks, ready, batchStage, batchOff, batchSize, cand, choice, crcOff, crcLen, crcOut;
     uint32_t* hostOne = nullptr;      // pinned constant 1 (chunk-arrival flags of the host-pointer path)
     uint64_t* hostSmall = nullptr;    // 256 pinned bytes the device writes its counters into (b2z_fetch_small)
@@ -64,3 +65,6 @@ int b2z_fetch_small(b200z_ctx* ctx, void* hostDst, const void* d_src, size_t byt
 // b2z_filter.cu: b200z_filter_device with units -- unitLog != 0 (encode only): the buffer is a run of independent units of 2^unitLog
 // bytes (the xz writer filters every Block on its own)
 int b2z_filter_units_device(b200z_ctx* ctx, uint32_t methodId, int encode, void* d_data, size_t n, uint32_t prop, uint32_t unitLog);
+
+// LZMA2 encoder: B200Z_E_PARAM (and last_error) unless lc + lp <= 4 and the model placement codes them; every compression entry checks it first
+int lz2_check_props(b200z_ctx* ctx);

@@ -89,7 +89,8 @@ enum : uint32_t {
 struct EncGeom;
 size_t lzma2_enc_slot_stride(const EncGeom& g);
 uint32_t lzma2_enc_slices_per_frame(const EncGeom& g);
-size_t lzma2_enc_model_bytes(uint32_t nChains);      // mode 3 (32 chains per warp): the chains' models, passed as litSpill
+size_t lzma2_enc_model_bytes(uint32_t nChains, uint32_t flags = 0);   // mode 3 (32 chains per warp): the chains' models, passed as litSpill
+uint32_t lzma2_enc_smem_chains_per_sm(uint32_t flags);     // chains per SM with the whole model in shared memory (modes 0 / 1)
 cudaError_t launch_lzma2_enc_range(const uint8_t* src, uint64_t srcSize, const EncGeom& g, const uint64_t* seqs, const uint32_t* nseq,
                                    uint8_t* slots, uint32_t* slotSize, uint32_t nFrames, uint16_t* litSpill, uint32_t smCount, int mode,
                                    uint32_t* status, cudaStream_t st);
@@ -100,7 +101,7 @@ void launch_lzma2_enc_assemble(const uint8_t* slots, const uint32_t* slotSize, u
 // ---- encoder, price-based parse (lzma2_parse.cu): stage C (candidates, one warp per frame; nWarps table sets) and stage P
 // (dynamic programme, one warp per state-reset slice) fill the per-block sequence arrays stage R reads
 size_t lzma2_cand_table_bytes(const EncGeom& g, uint32_t nWarps);
-size_t lzma2_parse_smem_bytes();
+size_t lzma2_parse_smem_bytes(uint32_t flags = 0);       // one warp's working set: grows with lc + lp (flags bits 15-23)
 void launch_lzma2_cand(const uint8_t* src, uint64_t srcSize, const EncGeom& g, uint32_t* tables, uint32_t nWarps, uint32_t* cand /* [srcSize * 4] */, cudaStream_t st);
 cudaError_t launch_lzma2_parse(const uint8_t* src, uint64_t srcSize, const EncGeom& g, const uint32_t* cand, uint64_t* seqs,
                                uint32_t* nseq /* one counter per 128 KiB block, zeroed here */, cudaStream_t st);

@@ -28,10 +28,22 @@
 #define LZM_L_LOW      2u
 #define LZM_L_MID      130u
 #define LZM_L_HIGH     258u
+/* the model at the compile-time context bits B2Z_LZ2_LC / LP / PB (the defaults, or what a statement compiled for one setting
+ * defines them as) */
 #define LZM_LITN       (0x300u << (B2Z_LZ2_LC + B2Z_LZ2_LP))
 #define LZM_NPROBS     (LZM_LIT + LZM_LITN)
 #define LZM_PBM        ((1u << B2Z_LZ2_PB) - 1u)
 #define LZM_LPM        ((1u << B2Z_LZ2_LP) - 1u)
+
+/* literal / position context bits of a coder (b2z_lz2_props: the LZMA2 properties byte).  Built from a constant byte, every
+ * function below folds them into its code.  The *_p functions take them; the ones without the suffix use B2Z_LZ2_LC / LP / PB. */
+typedef struct { uint32_t lc, lp, pb; } lzm_props;
+B2Z_HD lzm_props lzm_props_of(uint32_t props) { lzm_props q; q.lc = b2z_lz2_lc(props); q.lp = b2z_lz2_lp(props); q.pb = b2z_lz2_pb(props); return q; }
+B2Z_HD uint32_t lzm_litn(lzm_props q) { return 0x300u << (q.lc + q.lp); }
+B2Z_HD uint32_t lzm_nprobs(lzm_props q) { return LZM_LIT + lzm_litn(q); }
+B2Z_HD uint32_t lzm_pbm(lzm_props q) { return (1u << q.pb) - 1u; }
+/* first probability of the literal coder of the byte at pos after byte prev */
+B2Z_HD uint32_t lzm_lit_base(lzm_props q, uint32_t pos, uint32_t prev) { return LZM_LIT + 0x300u * (((pos & ((1u << q.lp) - 1u)) << q.lc) + (prev >> (8u - q.lc))); }
 
 /* price[i] = round(-16 * log2((16 i + 8) / 2048)), i = probability >> 4 */
 #define LZM_PRICE_LIST \
@@ -106,8 +118,8 @@ B2Z_HD uint32_t lzm_price_dist(const uint8_t *pt, const uint16_t *probs, uint32_
     return c;
 }
 /* the 8 bits of literal `sym` at pos after byte `prev`; matched = coded in a state >= 7 against byte mb (the byte at rep0) */
-B2Z_HD uint32_t lzm_price_literal(const uint8_t *pt, const uint16_t *probs, uint32_t pos, uint32_t prev, uint32_t sym, uint32_t matched, uint32_t mb) {
-    const uint16_t *p = probs + LZM_LIT + 0x300u * (((pos & LZM_LPM) << B2Z_LZ2_LC) + (prev >> (8u - B2Z_LZ2_LC)));
+B2Z_HD uint32_t lzm_price_literal_p(const uint8_t *pt, const uint16_t *probs, lzm_props q, uint32_t pos, uint32_t prev, uint32_t sym, uint32_t matched, uint32_t mb) {
+    const uint16_t *p = probs + lzm_lit_base(q, pos, prev);
     uint32_t c = 0, m = 1;
     for (uint32_t i = 8; i--;) {
         const uint32_t b = (sym >> i) & 1u;
@@ -116,6 +128,9 @@ B2Z_HD uint32_t lzm_price_literal(const uint8_t *pt, const uint16_t *probs, uint
         m = (m << 1) | b;
     }
     return c;
+}
+B2Z_HD uint32_t lzm_price_literal(const uint8_t *pt, const uint16_t *probs, uint32_t pos, uint32_t prev, uint32_t sym, uint32_t matched, uint32_t mb) {
+    return lzm_price_literal_p(pt, probs, lzm_props_of(B2Z_LZ2_PROPS), pos, prev, sym, matched, mb);
 }
 
 /* ---- the probability updates of one coded packet (what stage R does to its model while it codes the packet) */
@@ -129,9 +144,9 @@ B2Z_HD void lzm_update_len(uint16_t *l, uint32_t len, uint32_t ps) {
 }
 typedef struct { uint32_t state, rep[4]; } lzm_ctx;      /* coder state next to the probabilities */
 
-B2Z_HD void lzm_commit_literal(uint16_t *probs, lzm_ctx *x, uint32_t pos, uint32_t prev, uint32_t sym, uint32_t mb /* byte at rep0, used when state >= 7 */) {
-    lzm_update(probs + LZM_ISMATCH + x->state * 16u + (pos & LZM_PBM), 0);
-    uint16_t *p = probs + LZM_LIT + 0x300u * (((pos & LZM_LPM) << B2Z_LZ2_LC) + (prev >> (8u - B2Z_LZ2_LC)));
+B2Z_HD void lzm_commit_literal_p(uint16_t *probs, lzm_ctx *x, lzm_props q, uint32_t pos, uint32_t prev, uint32_t sym, uint32_t mb /* byte at rep0, used when state >= 7 */) {
+    lzm_update(probs + LZM_ISMATCH + x->state * 16u + (pos & lzm_pbm(q)), 0);
+    uint16_t *p = probs + lzm_lit_base(q, pos, prev);
     uint32_t m = 1, matched = x->state >= 7u;
     for (uint32_t i = 8; i--;) {
         const uint32_t b = (sym >> i) & 1u;
@@ -142,8 +157,8 @@ B2Z_HD void lzm_commit_literal(uint16_t *probs, lzm_ctx *x, uint32_t pos, uint32
     x->state = lzm_state_lit(x->state);
 }
 /* a match of len (2..273) at dist (= distance - 1): coded as the first rep that holds dist, else as a new distance (stage R's rule) */
-B2Z_HD void lzm_commit_match(uint16_t *probs, lzm_ctx *x, uint32_t pos, uint32_t len, uint32_t dist) {
-    const uint32_t ps = pos & LZM_PBM, s = x->state;
+B2Z_HD void lzm_commit_match_p(uint16_t *probs, lzm_ctx *x, lzm_props q, uint32_t pos, uint32_t len, uint32_t dist) {
+    const uint32_t ps = pos & lzm_pbm(q), s = x->state;
     lzm_update(probs + LZM_ISMATCH + s * 16u + ps, 1);
     const int r = dist == x->rep[0] ? 0 : (dist == x->rep[1] ? 1 : (dist == x->rep[2] ? 2 : (dist == x->rep[3] ? 3 : -1)));
     if (r < 0) {
@@ -173,5 +188,10 @@ B2Z_HD void lzm_commit_match(uint16_t *probs, lzm_ctx *x, uint32_t pos, uint32_t
         x->state = lzm_state_rep(s);
     }
 }
+
+B2Z_HD void lzm_commit_literal(uint16_t *probs, lzm_ctx *x, uint32_t pos, uint32_t prev, uint32_t sym, uint32_t mb) {
+    lzm_commit_literal_p(probs, x, lzm_props_of(B2Z_LZ2_PROPS), pos, prev, sym, mb);
+}
+B2Z_HD void lzm_commit_match(uint16_t *probs, lzm_ctx *x, uint32_t pos, uint32_t len, uint32_t dist) { lzm_commit_match_p(probs, x, lzm_props_of(B2Z_LZ2_PROPS), pos, len, dist); }
 
 #endif

@@ -61,10 +61,20 @@
 #define B2Z_SEQ_ML(s)      ((uint32_t)(((s) >> 46) & 0x3FFFFu))
 
 /* ---- LZMA2 encoder (stage R: range coding of the stage-M sequences of one frame = one dictionary-reset block) ---- */
+/* default literal / position context bits (B200Z_P_LZMA2_LC/LP/PB change them) */
 #define B2Z_LZ2_LC 2u      /* 2 codes G2 text as well as 3 (2.3961 vs 2.3955) and halves the literal model: the whole model fits shared memory */
 #define B2Z_LZ2_LP 0u
 #define B2Z_LZ2_PB 2u
 #define B2Z_LZ2_PROPS ((B2Z_LZ2_PB * 5u + B2Z_LZ2_LP) * 9u + B2Z_LZ2_LC)   /* 0x5D */
+/* flags bit 15: the coders take lc / lp / pb from the properties byte (pb * 5 + lp) * 9 + lc in flags bits 16..23 (lc + lp <= 4,
+ * pb <= 4) and run their run-time instantiations; clear: the defaults above, through the compile-time instantiations */
+#define B2Z_FLAG_LZ2_PROPS 0x8000u
+B2Z_HD uint32_t b2z_lz2_props(uint32_t flags) { return (flags & B2Z_FLAG_LZ2_PROPS) ? ((flags >> 16) & 0xFFu) : B2Z_LZ2_PROPS; }
+B2Z_HD uint32_t b2z_lz2_lc(uint32_t props) { return props % 9u; }
+B2Z_HD uint32_t b2z_lz2_lp(uint32_t props) { return (props / 9u) % 5u; }
+B2Z_HD uint32_t b2z_lz2_pb(uint32_t props) { return props / 45u; }
+/* literal model entries: 0x300 << (lc + lp) */
+B2Z_HD uint32_t b2z_lz2_litn(uint32_t props) { return 0x300u << (b2z_lz2_lc(props) + b2z_lz2_lp(props)); }
 #define B2Z_LZ2_PACK_LIMIT   (65536u - 64u)        /* a chunk is closed once this many packed bytes are pending (format max 64 KiB) */
 #define B2Z_LZ2_UNPACK_LIMIT ((1u << 21) - 512u)   /* ... or this many input bytes are covered (format max 2 MiB)                 */
 #define B2Z_LZ2_MAXLEN 273u

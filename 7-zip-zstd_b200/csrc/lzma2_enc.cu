@@ -76,7 +76,8 @@ __device__ __forceinline__ void rce_len(RcE& e, uint16_t* l, uint32_t len, uint3
 // L: chains per warp (lanes 0, 32/L, 2*32/L ... each run one chain).  Only L = 1 is launched: L = 2/4/8 measured
 // slower -- the chains' control flow diverges at every coded bit, so the hardware
 // serialises them and the shared convergent code does not pay for it.
-template <bool GLIT, int L>
+// DYN: lc / lp / pb from the properties byte in g.flags (B2Z_FLAG_LZ2_PROPS); otherwise the defaults, as compile-time constants
+template <bool GLIT, int L, bool DYN = false>
 // <= 64 registers: they are allocated for all 32 lanes of a chain's warp, so registers -- not shared memory -- bound the
 // chains per SM (32 at 64 registers)
 __global__ void __launch_bounds__(64, 16)
@@ -90,7 +91,8 @@ lzma2_enc_range_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
     const uint32_t slotInCta = (threadIdx.x >> 5) * (uint32_t)L + (threadIdx.x & 31u) / LSTEP;
     const uint32_t chain = blockIdx.x * (blockDim.x >> 5) * (uint32_t)L + slotInCta;
     if (chain >= nChains) return;
-    constexpr uint32_t LITN = 0x300u << (B2Z_LZ2_LC + B2Z_LZ2_LP);
+    const uint32_t props = DYN ? b2z_lz2_props(g.flags) : B2Z_LZ2_PROPS;
+    const uint32_t LC = b2z_lz2_lc(props), LITN = b2z_lz2_litn(props);
     uint16_t* const probs = probsAll + (size_t)slotInCta * (GLIT ? P_LIT : P_LIT + LITN);
     const uint64_t F = 1ull << g.frameLog;
     const uint32_t bpf = (uint32_t)(F >> 17), sliceBlocks = B2Z_LZ2_SLICE_BLOCKS(g.frameLog, g.flags), spf = bpf / sliceBlocks;
@@ -103,7 +105,7 @@ lzma2_enc_range_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
     uint16_t* lit = GLIT ? litSpill + (size_t)chain * LITN : probs + P_LIT;
     if (GLIT) asm volatile("" : "+l"(lit));                         // keep the base in registers: ptxas otherwise rebuilds it from the
                                                                     // kernel parameters at every probability access (5 instructions per bit)
-    constexpr uint32_t PBM = (1u << B2Z_LZ2_PB) - 1u, LPM = (1u << B2Z_LZ2_LP) - 1u;
+    const uint32_t PBM = (1u << b2z_lz2_pb(props)) - 1u, LPM = (1u << b2z_lz2_lp(props)) - 1u;
 
     RcE e; e.low = 0; e.range = 0; e.cacheSize = 0; e.cache = 0; e.out = slots + (size_t)chain * slotStride; e.op = 0;
     uint32_t state = 0, rep0 = 0, rep1 = 0, rep2 = 0, rep3 = 0;
@@ -125,7 +127,7 @@ lzma2_enc_range_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
             const uint32_t mode = needDict ? 3u : (needProps ? 2u : (needState ? 1u : 0u));
             h[0] = (uint8_t)(0x80u | (mode << 5) | ((unpack - 1u) >> 16)); h[1] = (uint8_t)((unpack - 1u) >> 8); h[2] = (uint8_t)(unpack - 1u);
             h[3] = (uint8_t)((pack - 1u) >> 8); h[4] = (uint8_t)(pack - 1u);
-            if (mode >= 2u) h[5] = (uint8_t)B2Z_LZ2_PROPS;
+            if (mode >= 2u) h[5] = (uint8_t)props;
             needDict = needProps = needState = false;
         }
         open = false;
@@ -154,7 +156,7 @@ lzma2_enc_range_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
     auto literal = [&]() {
         const uint32_t nxt = (pos + 1u < n) ? (uint32_t)__ldg(base + pos + 1u) : 0u;         // for the next packet
         rce_bit(e, probs + P_ISMATCH + state * 16u + (pos & PBM), 0);
-        uint16_t* p = lit + 0x300u * (((pos & LPM) << B2Z_LZ2_LC) + (prev >> (8u - B2Z_LZ2_LC)));
+        uint16_t* p = lit + 0x300u * (((pos & LPM) << LC) + (prev >> (8u - LC)));
         uint32_t m = 1, i = 8;
         if (state >= 7u) {                                          // matched literal: context follows the byte at rep0 while it agrees
 #pragma unroll 1
@@ -265,7 +267,8 @@ lzma2_enc_range_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
 #define B2Z_R32_DEPTH  4
 #define B2Z_R32_DIRECT 0x1FFFu   // "probability index" of a direct bit (range halves, no model)
 #define B2Z_R32_WARPS  2u
-static_assert(P_LIT + (0x300u << (B2Z_LZ2_LC + B2Z_LZ2_LP)) < B2Z_R32_DIRECT, "a queue entry holds a 13-bit probability index");
+#define B2Z_R32_MAX_LCLP 3u     // lc + lp of this kernel: its literal model must fit the 13-bit index (lc + lp = 4 is refused)
+static_assert(P_LIT + (0x300u << B2Z_R32_MAX_LCLP) < B2Z_R32_DIRECT, "a queue entry holds a 13-bit probability index");
 
 __device__ __forceinline__ void rce32_shift_low(RcE& e) {
     if ((uint32_t)e.low < 0xFF000000u || (uint32_t)(e.low >> 32) != 0u) {
@@ -280,13 +283,15 @@ __device__ __forceinline__ void rce32_shift_low(RcE& e) {
     e.low = (e.low & 0x00FFFFFFull) << 8;
 }
 
+template <bool DYN = false>     // as the kernel above
 __global__ void __launch_bounds__(32 * B2Z_R32_WARPS)
 lzma2_enc_range32_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g, const uint64_t* __restrict__ seqs,
                          const uint32_t* __restrict__ nseq, uint8_t* __restrict__ slots, uint32_t slotStride,
                          uint32_t* __restrict__ slotSize, uint16_t* models, uint32_t* __restrict__ status, uint32_t nChains) {
     B2Z_EXTERN_SMEM(uint16_t, queues);
-    constexpr uint32_t LITN = 0x300u << (B2Z_LZ2_LC + B2Z_LZ2_LP), NPROBS = P_LIT + LITN;
-    constexpr uint32_t PBM = (1u << B2Z_LZ2_PB) - 1u, LPM = (1u << B2Z_LZ2_LP) - 1u;
+    const uint32_t props = DYN ? b2z_lz2_props(g.flags) : B2Z_LZ2_PROPS;
+    const uint32_t LC = b2z_lz2_lc(props), NPROBS = P_LIT + b2z_lz2_litn(props);
+    const uint32_t PBM = (1u << b2z_lz2_pb(props)) - 1u, LPM = (1u << b2z_lz2_lp(props)) - 1u;
     const uint32_t lane = threadIdx.x & 31u, wic = threadIdx.x >> 5;
     const uint32_t group = blockIdx.x * (blockDim.x >> 5) + wic, chain = group * 32u + lane;
     uint16_t* const q = queues + (size_t)wic * B2Z_R32_QCAP * 32u + lane;                 // slot s of this lane: q[(s % QCAP) * 32]
@@ -333,7 +338,7 @@ lzma2_enc_range32_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncG
             const uint32_t mode = needDict ? 3u : (needProps ? 2u : (needState ? 1u : 0u));
             h[0] = (uint8_t)(0x80u | (mode << 5) | ((unpack - 1u) >> 16)); h[1] = (uint8_t)((unpack - 1u) >> 8); h[2] = (uint8_t)(unpack - 1u);
             h[3] = (uint8_t)((pack - 1u) >> 8); h[4] = (uint8_t)(pack - 1u);
-            if (mode >= 2u) h[5] = (uint8_t)B2Z_LZ2_PROPS;
+            if (mode >= 2u) h[5] = (uint8_t)props;
             needDict = needProps = needState = false;
         }
         open = false;
@@ -368,7 +373,7 @@ lzma2_enc_range32_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncG
     auto literal = [&]() {
         const uint32_t nxt = (pos + 1u < n) ? (uint32_t)__ldg(base + pos + 1u) : 0u;     // for the next packet
         put(P_ISMATCH + state * 16u + (pos & PBM), 0);
-        const uint32_t p = P_LIT + 0x300u * (((pos & LPM) << B2Z_LZ2_LC) + (prev >> (8u - B2Z_LZ2_LC)));
+        const uint32_t p = P_LIT + 0x300u * (((pos & LPM) << LC) + (prev >> (8u - LC)));
         uint32_t m = 1; bool matched = state >= 7u;                 // matched literal: the context follows the byte at rep0 while it agrees
 #pragma unroll
         for (int k = 7; k >= 0; k--) {                              // one shape for every lane: no early exit
@@ -535,34 +540,48 @@ size_t lzma2_enc_slot_stride(const EncGeom& g) {
     return ((size_t)B2Z_LZ2_FRAME_BOUND(sliceBytes) + 255u) & ~(size_t)255u;
 }
 
-// bytes of model memory the lock-step kernel needs for nChains chains (whole groups of 32)
-size_t lzma2_enc_model_bytes(uint32_t nChains) { return (size_t)((nChains + 31u) / 32u) * 32u * (P_LIT + (0x300u << (B2Z_LZ2_LC + B2Z_LZ2_LP))) * sizeof(uint16_t); }
+// bytes of model memory the lock-step kernel needs for nChains chains (whole groups of 32) with the properties of flags
+size_t lzma2_enc_model_bytes(uint32_t nChains, uint32_t flags) { return (size_t)((nChains + 31u) / 32u) * 32u * (P_LIT + b2z_lz2_litn(b2z_lz2_props(flags))) * sizeof(uint16_t); }
+// chains per SM whose whole model fits shared memory (one chain per CTA, 1 KiB reserved per CTA)
+uint32_t lzma2_enc_smem_chains_per_sm(uint32_t flags) {
+    return (uint32_t)((227u * 1024u) / (((size_t)P_LIT + b2z_lz2_litn(b2z_lz2_props(flags))) * sizeof(uint16_t) + 1024));
+}
 
 #ifndef B2Z_CUEMU
+template <bool DYN>
+static void launch_range_kernels(const uint8_t* src, uint64_t srcSize, const EncGeom& g, const uint64_t* seqs, const uint32_t* nseq,
+                                 uint8_t* slots, uint32_t stride, uint32_t* slotSize, uint32_t nChains, uint16_t* litSpill, int mode, bool glit,
+                                 size_t smemFull, uint32_t* status, cudaStream_t st, cudaError_t* err) {
+    if (mode == 3) {                                                // 32 chains per warp (experimental, see the kernel's header); litSpill holds whole models here (lzma2_enc_model_bytes)
+        const uint32_t groups = (nChains + 31u) / 32u;
+        lzma2_enc_range32_kernel<DYN><<<(groups + B2Z_R32_WARPS - 1u) / B2Z_R32_WARPS, 32 * B2Z_R32_WARPS, B2Z_R32_WARPS * B2Z_R32_QCAP * 32u * sizeof(uint16_t), st>>>(
+            src, srcSize, g, seqs, nseq, slots, stride, slotSize, litSpill, status, nChains);
+    } else if (glit) {     // two warps (chains) per CTA: 32 CTAs/SM would otherwise cap residency below the register limit
+        lzma2_enc_range_kernel<true, 1, DYN><<<(nChains + 1u) / 2u, 64, 2u * P_LIT * sizeof(uint16_t), st>>>(src, srcSize, g, seqs, nseq, slots, stride, slotSize, litSpill, status, nChains);
+    } else {
+        *err = cudaFuncSetAttribute(lzma2_enc_range_kernel<false, 1, DYN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemFull);
+        if (*err != cudaSuccess) return;
+        lzma2_enc_range_kernel<false, 1, DYN><<<nChains, 32, smemFull, st>>>(src, srcSize, g, seqs, nseq, slots, stride, slotSize, nullptr, status, nChains);
+    }
+}
+
 cudaError_t launch_lzma2_enc_range(const uint8_t* src, uint64_t srcSize, const EncGeom& g, const uint64_t* seqs, const uint32_t* nseq,
                                    uint8_t* slots, uint32_t* slotSize, uint32_t nFrames, uint16_t* litSpill, uint32_t smCount, int mode,
                                    uint32_t* status, cudaStream_t st) {
     if (!nFrames) return cudaSuccess;
-    constexpr uint32_t LITN = 0x300u << (B2Z_LZ2_LC + B2Z_LZ2_LP);
     const uint32_t nChains = nFrames * lzma2_enc_slices_per_frame(g);
-    const size_t smemFull = ((size_t)P_LIT + LITN) * sizeof(uint16_t);
-    const uint32_t slotsResident = (uint32_t)((227u * 1024u) / (smemFull + 1024)) * smCount;
+    const size_t smemFull = ((size_t)P_LIT + b2z_lz2_litn(b2z_lz2_props(g.flags))) * sizeof(uint16_t);
+    const uint32_t slotsResident = lzma2_enc_smem_chains_per_sm(g.flags) * smCount;
     // Literal model in global memory when the chains outnumber the shared-memory slots: more chains resident beat the ~6 extra
     // instructions per literal bit of the global-memory model.
     const bool glit = mode == 2 || (mode == 0 && litSpill && nChains > slotsResident);
     const uint32_t stride = (uint32_t)lzma2_enc_slot_stride(g);
-    if (mode == 3) {                                                // 32 chains per warp (experimental, see the kernel's header); litSpill holds whole models here (lzma2_enc_model_bytes)
-        if (!litSpill) return cudaErrorInvalidValue;
-        const uint32_t groups = (nChains + 31u) / 32u;
-        lzma2_enc_range32_kernel<<<(groups + B2Z_R32_WARPS - 1u) / B2Z_R32_WARPS, 32 * B2Z_R32_WARPS, B2Z_R32_WARPS * B2Z_R32_QCAP * 32u * sizeof(uint16_t), st>>>(
-            src, srcSize, g, seqs, nseq, slots, stride, slotSize, litSpill, status, nChains);
-    } else if (glit) {     // two warps (chains) per CTA: 32 CTAs/SM would otherwise cap residency below the register limit
-        lzma2_enc_range_kernel<true, 1><<<(nChains + 1u) / 2u, 64, 2u * P_LIT * sizeof(uint16_t), st>>>(src, srcSize, g, seqs, nseq, slots, stride, slotSize, litSpill, status, nChains);
-    } else {
-        cudaError_t e = cudaFuncSetAttribute(lzma2_enc_range_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemFull);
-        if (e != cudaSuccess) return e;
-        lzma2_enc_range_kernel<false, 1><<<nChains, 32, smemFull, st>>>(src, srcSize, g, seqs, nseq, slots, stride, slotSize, nullptr, status, nChains);
-    }
+    if (mode == 3 && (!litSpill || b2z_lz2_lc(b2z_lz2_props(g.flags)) + b2z_lz2_lp(b2z_lz2_props(g.flags)) > B2Z_R32_MAX_LCLP)) return cudaErrorInvalidValue;
+    cudaError_t e = cudaSuccess;
+    // the default properties run the compile-time instantiations; any other lc / lp / pb the run-time ones
+    if (g.flags & B2Z_FLAG_LZ2_PROPS) launch_range_kernels<true>(src, srcSize, g, seqs, nseq, slots, stride, slotSize, nChains, litSpill, mode, glit, smemFull, status, st, &e);
+    else launch_range_kernels<false>(src, srcSize, g, seqs, nseq, slots, stride, slotSize, nChains, litSpill, mode, glit, smemFull, status, st, &e);
+    if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }
 

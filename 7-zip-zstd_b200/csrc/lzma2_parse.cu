@@ -110,8 +110,7 @@ enum : uint32_t { PK_LIT = 0, PK_REP = 1, PK_MATCH = 2 };
 
 __constant__ uint8_t c_lzm_prices[128] = { LZM_PRICE_LIST };
 
-struct ParseSmem {                       // one warp's working set
-    uint16_t probs[LZM_NPROBS];
+struct ParseSmem {                       // one warp's working set; the model, lzm_nprobs() probabilities, follows it
     uint32_t cost[LZP_WIN + 1];
     uint32_t link[LZP_WIN + 1];          // best arrival: PLINK(from, len, kind, rep index)
     uint32_t dist[LZP_WIN + 1];          // ... its distance - 1 (PK_MATCH)
@@ -124,8 +123,10 @@ struct ParseSmem {                       // one warp's working set
     uint8_t  pt[128];
     uint32_t ctx[5];                     // committed coder state: state, rep0..3
 };
-size_t lzma2_parse_smem_bytes() { return sizeof(ParseSmem); }
+size_t lzma2_parse_smem_bytes(uint32_t flags) { return sizeof(ParseSmem) + (size_t)lzm_nprobs(lzm_props_of(b2z_lz2_props(flags))) * sizeof(uint16_t); }
 
+// DYN: lc / lp / pb from the properties byte in g.flags (B2Z_FLAG_LZ2_PROPS); otherwise the defaults, as compile-time constants
+template <bool DYN = false>
 __global__ void __launch_bounds__(32)
 lzma2_parse_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g, const uint32_t* __restrict__ cand,
                    uint64_t* __restrict__ seqs, uint32_t* __restrict__ nseq, uint32_t nChains) {
@@ -146,10 +147,11 @@ lzma2_parse_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
     uint64_t* const fseqs = seqs + (size_t)f * bpf * B2Z_MAXSEQ;
     uint32_t* const fnseq = nseq + (size_t)f * bpf;
     const uint8_t* const pt = S->pt;
-    uint16_t* const probs = S->probs;
+    uint16_t* const probs = reinterpret_cast<uint16_t*>(S + 1);
+    const lzm_props q = lzm_props_of(DYN ? b2z_lz2_props(g.flags) : B2Z_LZ2_PROPS);
 
     for (uint32_t k = lane; k < 128u; k += 32u) S->pt[k] = c_lzm_prices[k];
-    for (uint32_t k = lane; k < LZM_NPROBS; k += 32u) probs[k] = 1024;
+    for (uint32_t k = lane; k < lzm_nprobs(q); k += 32u) probs[k] = 1024;
     if (lane < 5u) S->ctx[lane] = 0;
     __syncwarp();
 
@@ -195,7 +197,7 @@ lzma2_parse_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
                 if (lane == 0) { S->state[i] = (uint8_t)st; S->rep[i][0] = r0; S->rep[i][1] = r1; S->rep[i][2] = r2; S->rep[i][3] = r3; }
             }
             if (i == W || (i && i == end)) break;
-            const uint32_t p = pos + i, ps = p & LZM_PBM;
+            const uint32_t p = pos + i, ps = p & lzm_pbm(q);
             const uint32_t maxLen = (s1 - p) < B2Z_LZ2_MAXLEN ? (s1 - p) : B2Z_LZ2_MAXLEN;
             const uint32_t lim32 = maxLen < 32u ? maxLen : 32u;
             const uint32_t curB = S->win[i + 1u + lane];             // frame byte p + lane (zero past the slice end: never compared there)
@@ -251,7 +253,7 @@ lzma2_parse_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
                     const uint32_t sh = 8u - lane, b = (sym >> (7u - lane)) & 1u;
                     const uint32_t m = (1u << lane) | (sym >> sh);
                     const bool matched = st >= 7u && (sym >> sh) == (mb >> sh);
-                    const uint16_t* lp = probs + LZM_LIT + 0x300u * (((p & LZM_LPM) << B2Z_LZ2_LC) + (prev >> (8u - B2Z_LZ2_LC)));
+                    const uint16_t* lp = probs + lzm_lit_base(q, p, prev);
                     const uint32_t mbit = (mb >> (7u - lane)) & 1u;
                     bitPrice = lzm_price(pt, matched ? lp[((1u + mbit) << 8) + m] : lp[m], b);
                 }
@@ -320,14 +322,14 @@ lzma2_parse_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
             for (uint32_t j = i; j > 0u; j = PLINK_FROM(S->link[j])) S->path[np++] = (uint16_t)j;
             while (np--) {
                 const uint32_t j = S->path[np], lk = S->link[j], fr = PLINK_FROM(lk), kind = PLINK_KIND(lk), p = pos + fr;
-                if (kind == PK_LIT) lzm_commit_literal(probs, &x, p, S->win[fr], S->win[fr + 1u], S->litMb[fr]);
+                if (kind == PK_LIT) lzm_commit_literal_p(probs, &x, q, p, S->win[fr], S->win[fr + 1u], S->litMb[fr]);
                 else {
                     const uint32_t d = kind == PK_MATCH ? S->dist[j] : x.rep[PLINK_R(lk)], len = PLINK_LEN(lk);
-                    lzm_commit_match(probs, &x, p, len, d);
+                    lzm_commit_match_p(probs, &x, q, p, len, d);
                     sink(p, len, d);
                 }
             }
-            if (longLen) { lzm_commit_match(probs, &x, pos + i, longLen, longDist); sink(pos + i, longLen, longDist); }
+            if (longLen) { lzm_commit_match_p(probs, &x, q, pos + i, longLen, longDist); sink(pos + i, longLen, longDist); }
             S->ctx[0] = x.state; S->ctx[1] = x.rep[0]; S->ctx[2] = x.rep[1]; S->ctx[3] = x.rep[2]; S->ctx[4] = x.rep[3];
         }
         __syncwarp();
@@ -354,10 +356,17 @@ cudaError_t launch_lzma2_parse(const uint8_t* src, uint64_t srcSize, const EncGe
     const size_t nBlocks = (size_t)(nFrames - 1u) * (size_t)(F >> 17) + (size_t)((lastBytes + B2Z_BLOCK - 1u) / B2Z_BLOCK);
     cudaError_t e = cudaMemsetAsync(nseq, 0, nBlocks * sizeof(uint32_t), st);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(lzma2_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ParseSmem));
-    if (e != cudaSuccess) return e;
+    const size_t smem = lzma2_parse_smem_bytes(g.flags);
     const uint32_t nChains = nFrames * lzma2_enc_slices_per_frame(g);
-    lzma2_parse_kernel<<<nChains, 32, sizeof(ParseSmem), st>>>(src, srcSize, g, cand, seqs, nseq, nChains);
+    if (g.flags & B2Z_FLAG_LZ2_PROPS) {                             // lc / lp / pb other than the defaults: the run-time instantiation
+        e = cudaFuncSetAttribute(lzma2_parse_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        lzma2_parse_kernel<true><<<nChains, 32, smem, st>>>(src, srcSize, g, cand, seqs, nseq, nChains);
+    } else {
+        e = cudaFuncSetAttribute(lzma2_parse_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        lzma2_parse_kernel<false><<<nChains, 32, smem, st>>>(src, srcSize, g, cand, seqs, nseq, nChains);
+    }
     return cudaGetLastError();
 }
 #endif

@@ -223,6 +223,7 @@ int b200z_xz_compress_host(b200z_ctx* ctx, const void* src, size_t n, void* dst,
     if (!ctx || !out || (!src && n) || !dst) return B200Z_E_PARAM;
     if (checkType != 0 && checkType != 1 && checkType != 4) return fail(ctx, B200Z_E_PARAM, "xz: check type must be 0 (none), 1 (CRC32) or 4 (CRC64)%s");
     if (filterId && !xz_filter_id(filterId)) return fail(ctx, B200Z_E_UNSUPPORTED, "xz: filter not built on the GPU%s");
+    { const int prc = lz2_check_props(ctx); if (prc) return prc; }   // lc / lp / pb travel in the chunk headers: no Block Header field for them
     if (cap < b200z_xz_compress_bound(ctx, n)) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_xz_compress_bound%s");
     CU(cudaSetDevice(ctx->device));
     const size_t lzCap = b200z_lzma2_compress_bound(ctx, n);

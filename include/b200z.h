@@ -73,6 +73,11 @@ extern "C" {
                                    sliding-window frame the reference's encoder writes (default), 2 = every frame (tests) */
 #define B200Z_P_DEC_JUMP_SEGLOG 17 /* stage J resolves the output in segments of 2^this bytes, in order (16..30, default 30: 4 GiB of pointers at most, frames of any size) */
 #define B200Z_P_HOST_BATCH_LOG 8 /* log2 of bytes per H2D|kernels|D2H pipeline batch of the *_host calls, default 30 (the decoder takes twice that) */
+#define B200Z_P_LZMA2_LC    18  /* LZMA2 encoder: literal context bits lc, 0..4 (default 2)                                                       */
+#define B200Z_P_LZMA2_LP    19  /* LZMA2 encoder: literal position bits lp, 0..4 (default 0); lc + lp <= 4 is checked when a compression starts   */
+#define B200Z_P_LZMA2_PB    20  /* LZMA2 encoder: position bits pb, 0..4 (default 2).  lc/lp/pb travel in the chunk headers' properties byte
+                                   (pb * 5 + lp) * 9 + lc; values other than 2/0/2 run the run-time instantiations of stages P and R.
+                                   LZMA2_MODEL 3 codes lc + lp <= 3 only.  The reference's encoders default to lc3 (lc2 codes text as well here) */
 
 /* statistics (b200z_get_stat): device milliseconds accumulated since the last b200z_reset_stats,
  * measured with CUDA events on the context's stream around each stage */
@@ -182,7 +187,8 @@ int b200z_lzma2_decompress_host(b200z_ctx *ctx, const void *src, size_t srcSize,
  * and returns the 1-byte coder property for the 7z folder (what ICompressWriteCoderProperties emits,
  * Lzma2Encoder.cpp:117-121 / FastLzma2 :353-364).  Replaces NCompress::NLzma2::CEncoder::Code -> Lzma2Enc_Encode2
  * (Lzma2Encoder.cpp:124-134, C/Lzma2Enc.c:717) and CFastEncoder::Code -> FL2_compressStream (Lzma2Encoder.cpp:280-340,
- * C/fast-lzma2/fl2_compress.c).  lc/lp/pb are fixed at 2/0/2. */
+ * C/fast-lzma2/fl2_compress.c).  lc/lp/pb are B200Z_P_LZMA2_LC/LP/PB (default 2/0/2); B200Z_E_PARAM when lc + lp > 4, or with
+ * B200Z_P_LZMA2_MODEL 3 when lc + lp > 3 (Lzma2Enc_SetProps, Lzma2Enc.c:471). */
 size_t b200z_lzma2_compress_bound(b200z_ctx *ctx, size_t srcSize);
 int b200z_lzma2_compress_device(b200z_ctx *ctx, const void *d_src, size_t srcSize, void *d_dst, size_t dstCap,
                                 size_t *dstSize, uint32_t *dictProp);
