@@ -103,9 +103,11 @@ __device__ SeqHdr parse_seq_hdr(const Src& S, uint64_t off, uint32_t avail) {
 //   D0b (thread/frame)  frame header + block count (and end-offset check)
 //   D0c (1 thread)      firstBlock = exclusive scan of the block counts
 //   D0d (thread/frame)  block table entries incl. where each block's entropy tables come from
-struct FrameHdr { uint64_t contentSize, windowSize; uint32_t checksum, hdrBytes, status; };
+// Block_Maximum_Size = min(Window_Size, 128 KiB) (RFC 8878 3.1.1.2.4)
+__device__ __forceinline__ uint64_t block_max(uint64_t windowSize) { return windowSize < 131072u ? windowSize : 131072u; }
+struct FrameHdr { uint64_t contentSize, windowSize, blockMax; uint32_t checksum, hdrBytes, status; };     // blockMax: from the declared window
 __device__ FrameHdr parse_frame_hdr(const Src& S, uint64_t ip, uint64_t srcSize) {
-    FrameHdr h; h.status = 0; h.contentSize = ~0ull; h.windowSize = 0; h.checksum = 0; h.hdrBytes = 0;
+    FrameHdr h; h.status = 0; h.contentSize = ~0ull; h.windowSize = 0; h.blockMax = 0; h.checksum = 0; h.hdrBytes = 0;
     if (srcSize - ip < 6) { h.status = B2Z_DERR_CORRUPT; return h; }
     const uint64_t ip0 = ip;
     const uint32_t fhd = S.u8(ip + 4); ip += 5;
@@ -126,7 +128,8 @@ __device__ FrameHdr parse_frame_hdr(const Src& S, uint64_t ip, uint64_t srcSize)
     if (fcsBytes) { uint64_t fcs = 0; for (uint32_t i = 0; i < fcsBytes; i++) fcs |= (uint64_t)S.u8(ip + i) << (8 * i); if (fcsBytes == 2) fcs += 256; h.contentSize = fcs; }
     ip += fcsBytes;
     if (single) h.windowSize = h.contentSize;
-    else if (h.contentSize != ~0ull && h.contentSize < h.windowSize) h.windowSize = h.contentSize;     // no offset can exceed the content (zstd --long=31 on a small file)
+    h.blockMax = block_max(h.windowSize);
+    if (!single && h.contentSize != ~0ull && h.contentSize < h.windowSize) h.windowSize = h.contentSize;     // no offset can exceed the content (zstd --long=31 on a small file)
     if (h.windowSize > (1ull << 30) - 16) { h.status = B2Z_DERR_UNSUPPORTED; return h; }
     h.hdrBytes = (uint32_t)(ip - ip0);
     return h;
@@ -134,14 +137,15 @@ __device__ FrameHdr parse_frame_hdr(const Src& S, uint64_t ip, uint64_t srcSize)
 
 // Walk the block headers of one frame starting at `ip` (first block header). Returns the status; *nb = blocks,
 // *ipEnd = offset after the last block.  With `out` != null also fills the block entries.
-__device__ uint32_t walk_blocks(const Src& S, uint64_t ip, uint64_t srcSize, uint32_t* nbOut, uint64_t* ipEnd,
+// blockMax: Block_Maximum_Size; no block's size field may exceed it.
+__device__ uint32_t walk_blocks(const Src& S, uint64_t ip, uint64_t srcSize, uint64_t blockMax, uint32_t* nbOut, uint64_t* ipEnd,
                                 DecBlock* out, uint32_t firstBlock, uint32_t frameIdx, uint32_t blockCap, uint32_t firstSlot = 0, uint32_t* nCompOut = nullptr) {
     uint32_t nb = 0, nComp = 0; int32_t lastHuf = -1, lastTbl[3] = { -1, -1, -1 };
     for (;;) {
         if (srcSize < ip || srcSize - ip < 3) return B2Z_DERR_CORRUPT;
         const uint32_t bh = S.le24(ip); ip += 3;
         const uint32_t last = bh & 1u, type = (bh >> 1) & 3u, bsize = bh >> 3;
-        if (type == 3 || bsize > 131072u) return B2Z_DERR_CORRUPT;
+        if (type == 3 || bsize > 131072u || bsize > blockMax) return B2Z_DERR_CORRUPT;
         const uint32_t cSize = type == 1 ? 1u : bsize;
         if (srcSize - ip < cSize) return B2Z_DERR_CORRUPT;
         if (out) {
@@ -210,7 +214,7 @@ __global__ void zstd_dec_find_frames_kernel(const uint8_t* __restrict__ src, uin
         const FrameHdr h = parse_frame_hdr(S, ip, srcSize);
         if (h.status) { status = h.status; break; }
         uint32_t nb; uint64_t end;
-        status = walk_blocks(S, ip + h.hdrBytes, srcSize, &nb, &end, nullptr, 0, nf, 0);
+        status = walk_blocks(S, ip + h.hdrBytes, srcSize, h.blockMax, &nb, &end, nullptr, 0, nf, 0);
         if (status) break;
         if (h.checksum) { if (srcSize - end < 4) { status = B2Z_DERR_CORRUPT; break; } end += 4; }
         DecFrame fr; fr.srcOff = ip; fr.dstOff = 0; fr.contentSize = ~0ull; fr.windowSize = 0; fr.regen = end; fr.firstBlock = 0; fr.nBlocks = nb; fr.checksum = 0; fr.pad = 0; fr.endOff = end; fr.jump = 0; fr.nComp = 0; fr.firstSlot = 0; fr.pad4 = 0;
@@ -227,7 +231,7 @@ __global__ void zstd_dec_count_blocks_kernel(const uint8_t* __restrict__ src, ui
     DecFrame fr = frames[f];
     const FrameHdr h = parse_frame_hdr(S, fr.srcOff, srcSize);
     uint32_t status = h.status, nb = 0, nComp = 0; uint64_t end = 0;
-    if (!status) status = walk_blocks(S, fr.srcOff + h.hdrBytes, srcSize, &nb, &end, nullptr, 0, f, 0, 0, &nComp);
+    if (!status) status = walk_blocks(S, fr.srcOff + h.hdrBytes, srcSize, h.blockMax, &nb, &end, nullptr, 0, f, 0, 0, &nComp);
     if (!status && h.checksum) { if (srcSize - end < 4) status = B2Z_DERR_CORRUPT; else end += 4; }
     if (!status && end != fr.regen) status = B2Z_DERR_CORRUPT;          // a size hint that does not match its frame
     fr.contentSize = h.contentSize; fr.windowSize = h.windowSize; fr.checksum = h.checksum; fr.nBlocks = nb; fr.pad = h.hdrBytes; fr.nComp = nComp;
@@ -253,7 +257,8 @@ __global__ void zstd_dec_fill_blocks_kernel(const uint8_t* __restrict__ src, uin
     Src S; S.w = reinterpret_cast<const uint64_t*>(src); S.nWords = (srcSize + 7) >> 3; S.size = srcSize;
     const DecFrame fr = frames[f];
     uint32_t nb; uint64_t end;
-    const uint32_t status = walk_blocks(S, fr.srcOff + fr.pad, srcSize, &nb, &end, blocks, fr.firstBlock, f, blockCap, fr.firstSlot);
+    const uint64_t blockMax = parse_frame_hdr(S, fr.srcOff, srcSize).blockMax;           // (fr.windowSize may be cut to the content size)
+    const uint32_t status = walk_blocks(S, fr.srcOff + fr.pad, srcSize, blockMax, &nb, &end, blocks, fr.firstBlock, f, blockCap, fr.firstSlot);
     frames[f].regen = 0; frames[f].pad = 0;
     if (status) atomicOr(&counts->status, status);
 }
@@ -770,6 +775,7 @@ __global__ void zstd_dec_frame_sizes_kernel(DecFrame* frames, uint32_t nFrames, 
         DecBlock& B = blocks[b0 + i];
         B.outRel = total; B.repInit[0] = r0; B.repInit[1] = r1; B.repInit[2] = r2;
         total += B.regen; st |= B.status;
+        if (B.regen > block_max(frames[f].windowSize)) st |= B2Z_DERR_CORRUPT;                // a compressed block decodes to at most Block_Maximum_Size
         if (i && i % B2Z_DEC_UNIT_BLOCKS == 0u) {                             // a unit's first block: does it copy from the unit before it?
             if (B.type == 2 && B.nearBehind) { chained++; run++; if (run > longest) longest = run; } else run = 0;
         }

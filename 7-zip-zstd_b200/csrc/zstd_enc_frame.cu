@@ -117,7 +117,9 @@ zstd_enc_gather_kernel(uint64_t srcSize, EncGeom g, const uint8_t* __restrict__ 
             kp[0] = 0x50; kp[1] = 0x2A; kp[2] = 0x4D; kp[3] = 0x18; kp[4] = 4; kp[5] = 0; kp[6] = 0; kp[7] = 0;
             kp[8] = (uint8_t)fsize; kp[9] = (uint8_t)(fsize >> 8); kp[10] = (uint8_t)(fsize >> 16); kp[11] = (uint8_t)(fsize >> 24);
         }
-        uint32_t wl = 10; while ((1ull << wl) < fn && wl < g.windowLog) wl++;
+        // the declared window covers the match distances (windowLog) and at least one whole block (RFC 8878 3.1.1.2.4: no block may
+        // exceed the window), so a window_log below 17 still declares min(frame, 128 KiB)
+        uint32_t wl = 10; while ((1ull << wl) < fn && (wl < g.windowLog || wl < 17u)) wl++;
         hp[0] = 0x28; hp[1] = 0xB5; hp[2] = 0x2F; hp[3] = 0xFD;
         hp[4] = (uint8_t)(0x80u | ((g.flags & 2u) ? 4u : 0u));
         hp[5] = (uint8_t)((wl - 10u) << 3);

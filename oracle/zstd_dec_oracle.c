@@ -434,6 +434,7 @@ int64_t b2zo_zstd_decompress(void *dstv, size_t dstCap, const void *srcv, size_t
             if (iend - ip < 3) { rc = -1; goto done; }
             uint32_t bh = ip[0] | (ip[1] << 8) | (ip[2] << 16); ip += 3;
             uint32_t last = bh & 1, type = (bh >> 1) & 3, bsize = bh >> 3;
+            if (bsize > blockMax) { rc = -1; goto done; }      /* RFC 8878 3.1.1.2.4: Block_Maximum_Size = min(Window_Size, 128 KiB) */
             if (type == 0) {
                 if ((size_t)(iend - ip) < bsize) { rc = -1; goto done; }
                 if ((size_t)(oend - op) < bsize) { rc = -2; goto done; }
@@ -449,7 +450,7 @@ int64_t b2zo_zstd_decompress(void *dstv, size_t dstCap, const void *srcv, size_t
                 size_t cap = (size_t)(oend - op) < ZF_BLOCK_MAX ? (size_t)(oend - op) : ZF_BLOCK_MAX;
                 int64_t r = decode_block(c, op, cap, frameStart, ip, bsize, (size_t)windowSize);
                 if (r < 0) { rc = ((size_t)(oend - op) < ZF_BLOCK_MAX && r == -2) ? -2 : (r == -2 ? -1 : r); goto done; }
-                if ((size_t)r > blockMax && !single) { /* tolerated: window-limited block size not enforced */ }
+                if ((size_t)r > blockMax) { rc = -1; goto done; }  /* nor may a compressed block decode to more */
                 op += r; ip += bsize;
             } else { rc = -1; goto done; }
             if (last) break;

@@ -648,7 +648,7 @@ static size_t compress_block(uint8_t *dst, const uint8_t *frame, size_t blkStart
 static size_t write_frame_header(uint8_t *dst, size_t n, const b2zo_enc_params *P) {
     wr32(dst, ZF_MAGIC);
     if (n == 0) { dst[4] = (uint8_t)(0x20 | ((P->flags & 2) ? 4 : 0)); dst[5] = 0; return 6; }     /* single segment, FCS = 0 */
-    uint32_t wl = 10; while (((size_t)1 << wl) < n && wl < P->windowLog) wl++;
+    uint32_t wl = 10; while (((size_t)1 << wl) < n && (wl < P->windowLog || wl < 17)) wl++;     /* >= min(frame, 128 KiB): whole blocks */
     dst[4] = (uint8_t)(0x80 | ((P->flags & 2) ? 4 : 0));     /* 4-byte FCS, window descriptor present */
     dst[5] = (uint8_t)((wl - 10) << 3);
     wr32(dst + 6, (uint32_t)n);
