@@ -69,7 +69,7 @@ struct DecCounts { uint32_t nFrames, nBlocks, status, nUnits; uint64_t srcUsed; 
 void launch_zstd_dec_find_frames(const uint8_t* src, uint64_t srcSize, DecFrame* frames, uint32_t frameCap, DecCounts* counts, bool useHints, cudaStream_t st);
 void launch_zstd_dec_index_blocks(const uint8_t* src, uint64_t srcSize, DecFrame* frames, uint32_t nFrames,
                                   DecBlock* blocks, uint32_t blockCap, DecCounts* counts, cudaStream_t st);
-// stage D1: tables (one warp per block) then streams (one thread per stream); literals | sequences on two CUDA streams
+// stage D1: headers, then streams (one thread per stream, decoding tables built in shared memory); literals | sequences on two CUDA streams
 void launch_zstd_dec_entropy(const uint8_t* src, uint64_t srcSize, DecBlock* blocks, uint32_t nBlocks,
                              uint8_t* lits, uint64_t* seqs, void* scratch, uint32_t smCount, cudaStream_t st, cudaStream_t stLit, cudaEvent_t evFork, cudaEvent_t evJoin);
 size_t zstd_dec_entropy_scratch_bytes(uint32_t nBlocks);

@@ -4,8 +4,8 @@
 //   D0 prepass  (1 thread)          walk frame and block headers (sequential by format), record
 //                                   per block where its entropy tables come from (treeless
 //                                   literals / repeat-mode FSE tables chain back to an earlier block)
-//   D1 entropy  (1 warp / block)    Huffman-decode the literals (4 streams -> 4 lanes) and FSE-decode
-//                                   the sequences (one backward bitstream -> lane 0) into scratch
+//   D1 entropy  (thread / stream)   Huffman-decode the literals (4 streams -> 4 threads) and FSE-decode
+//                                   the sequences (one backward bitstream -> 1 thread), tables in shared memory
 //   D2 layout   (1 thread / frame)  block sizes -> frame sizes -> output offsets
 //   D3 execute  (1 warp / frame)    literal + match copies, block after block (matches may reach
 //                                   into earlier blocks of the frame), repcode history carried
@@ -303,20 +303,13 @@ struct BwdBits {                                // backward stream with end mark
     }
 };
 
-// ---------------------------------------------------------------- per-warp workspace of D1
-struct SeqEnt { uint32_t base; uint8_t nbAdd, nbBits; uint16_t next; };
-// ROLE 0 = literals kernel (needs the Huffman table), ROLE 1 = sequences kernel (needs the three FSE tables)
-template <int ROLE> struct DecWST {
-    uint16_t huf[ROLE == 0 ? 2048 : 64];     // symbol | nbBits << 8
-    SeqEnt   tabs[ROLE == 1 ? 1280 : 1];     // LL [0,512), OF [512,768), ML [768,1280)
-    __device__ __forceinline__ SeqEnt* tab(int t) { return tabs + (t == 0 ? 0 : (t == 1 ? 512 : 768)); }
-    __device__ __forceinline__ const SeqEnt* tab(int t) const { return tabs + (t == 0 ? 0 : (t == 1 ? 512 : 768)); }
-    uint32_t tabLog[3];
-    uint32_t hufBits;
-    int16_t  norm[256];
-    uint16_t nxt[256];
-    uint8_t  sym[512];           // FSE symbol per state (build scratch) / Huffman weights
-};
+// ---------------------------------------------------------------- D1 tables (built on chip, one thread per block)
+// Sequence decoding tables of one block: LL [0,512) | OF [512,768) | ML [768,1280) entries of 16 bits, symbol | ns << 6, where ns
+// is FSE_buildDTable's per-symbol state counter (< 2^10): the state's nbBits = log - highbit(ns) and its next-state base =
+// (ns << nbBits) - 2^log.  The baseline and the number of extra bits follow from the symbol (k_seqSym below for LL and ML;
+// 1 << s and s for OF).  Two bytes per state keep 2.5 KiB per block in shared memory.
+#define B2Z_SEQ_TAB 1280u
+__device__ __forceinline__ uint32_t seq_tab_off(int t) { return t == 0 ? 0u : (t == 1 ? 512u : 768u); }
 
 // FSE normalized counts; returns bytes consumed or 0
 __device__ uint32_t fse_read_ncount(int16_t* norm, uint32_t* maxSym, uint32_t* tableLog, const Src& S, uint64_t off, uint32_t size, uint32_t maxLog) {
@@ -349,36 +342,23 @@ __device__ uint32_t fse_read_ncount(int16_t* norm, uint32_t* maxSym, uint32_t* t
     return used;
 }
 
-// generic FSE decode table: symbol per state in ws->sym, (nbBits, newState) returned through arrays
-template <class WS> __device__ bool fse_spread(WS* ws, const int16_t* norm, uint32_t maxSym, uint32_t log) {
+// FSE decoding table into tab[0, 2^log) (seq_tab_off's layout); norm[] is consumed (it ends as the state counters).  false when
+// the spread does not close (malformed counts)
+__device__ bool build_seq_table(uint16_t* tab, int16_t* norm, uint32_t maxSym, uint32_t log) {
     const uint32_t size = 1u << log, mask = size - 1u; uint32_t high = size - 1u;
-    for (uint32_t s = 0; s <= maxSym; s++) {
-        if (norm[s] == -1) { ws->sym[high--] = (uint8_t)s; ws->nxt[s] = 1; } else ws->nxt[s] = (uint16_t)norm[s];
-    }
+    for (uint32_t s = 0; s <= maxSym; s++) if (norm[s] == -1) tab[high--] = (uint16_t)s;
     const uint32_t step = (size >> 1) + (size >> 3) + 3u; uint32_t pos = 0;
     for (uint32_t s = 0; s <= maxSym; s++)
-        for (int i = 0; i < norm[s]; i++) { ws->sym[pos] = (uint8_t)s; pos = (pos + step) & mask; while (pos > high) pos = (pos + step) & mask; }
-    return pos == 0;
-}
-
-template <class WS> __device__ bool build_seq_table(WS* ws, int t, const int16_t* norm, uint32_t maxSym, uint32_t log) {
-    if (!fse_spread(ws, norm, maxSym, log)) return false;
-    const uint32_t size = 1u << log;
-    for (uint32_t u = 0; u < size; u++) {
-        const uint32_t s = ws->sym[u], ns = ws->nxt[s]++;
-        SeqEnt e; e.nbBits = (uint8_t)(log - highbit32(ns)); e.next = (uint16_t)((ns << e.nbBits) - size);
-        if (t == 0) { e.base = k_LL_base[s]; e.nbAdd = k_LL_bits[s]; }
-        else if (t == 2) { e.base = k_ML_base[s]; e.nbAdd = k_ML_bits[s]; }
-        else { e.base = 1u << s; e.nbAdd = (uint8_t)s; }
-        ws->tab(t)[u] = e;
-    }
-    ws->tabLog[t] = log;
+        for (int i = 0; i < norm[s]; i++) { tab[pos] = (uint16_t)s; pos = (pos + step) & mask; while (pos > high) pos = (pos + step) & mask; }
+    if (pos != 0) return false;
+    for (uint32_t s = 0; s <= maxSym; s++) if (norm[s] == -1) norm[s] = 1;
+    for (uint32_t u = 0; u < size; u++) { const uint32_t s = tab[u], ns = (uint32_t)norm[s]++; tab[u] = (uint16_t)(s | (ns << 6)); }
     return true;
 }
 
 // Walk the table descriptions of block `blk`'s sequences section; returns the offset (absolute in src)
-// and mode of type t's description.  false on malformed data.
-template <class WS> __device__ bool locate_seq_table(const Src& S, const DecBlock& blk, int t, WS* ws, uint64_t* descOff, uint32_t* mode, uint32_t* avail) {
+// and mode of type t's description.  false on malformed data.  norm: scratch of 53 counts
+__device__ bool locate_seq_table(const Src& S, const DecBlock& blk, int t, int16_t* norm, uint64_t* descOff, uint32_t* mode, uint32_t* avail) {
     const LitHdr lh = parse_lit_hdr(S, blk.srcOff, blk.cSize);
     if (!lh.ok) return false;
     const uint32_t so = lh.hdr + lh.csize;
@@ -391,17 +371,18 @@ template <class WS> __device__ bool locate_seq_table(const Src& S, const DecBloc
         if (k == t) { *descOff = p; *mode = m; *avail = left; return true; }
         uint32_t used = 0;
         if (m == 1) used = 1;
-        else if (m == 2) { uint32_t ms = maxSymT[k], lg; used = fse_read_ncount(ws->norm, &ms, &lg, S, p, left, maxLogT[k]); if (!used) return false; }
+        else if (m == 2) { uint32_t ms = maxSymT[k], lg; used = fse_read_ncount(norm, &ms, &lg, S, p, left, maxLogT[k]); if (!used) return false; }
         if (used > left) return false;
         p += used; left -= used;
     }
     return false;
 }
 
-// Huffman decoding table from the description at `off`; returns description bytes or 0
-template <class WS> __device__ uint32_t huf_read_table(WS* ws, const Src& S, uint64_t off, uint32_t size) {
+// Huffman weights of the description at `off` into w[0, *nw) (the last, implied weight included), checked as a complete code;
+// returns the description's bytes and *maxBits, or 0.  One thread; its scratch lives in its own frame.
+__device__ __forceinline__ uint32_t huf_read_weights(uint8_t* w, uint32_t* nwOut, uint32_t* maxBitsOut, const Src& S, uint64_t off, uint32_t size) {
     if (size < 1) return 0;
-    uint8_t* w = ws->sym; uint32_t nw = 0;
+    uint32_t nw = 0;
     const uint32_t hb = S.u8(off); uint32_t used;
     if (hb >= 128) {
         nw = hb - 127u; used = 1u + (nw + 1u) / 2u;
@@ -410,22 +391,23 @@ template <class WS> __device__ uint32_t huf_read_table(WS* ws, const Src& S, uin
     } else {
         used = 1u + hb;
         if (hb == 0 || used > size) return 0;
+        int16_t norm[256]; uint16_t nxt[256];
         uint32_t maxSym = 255, al;
-        const uint32_t hs = fse_read_ncount(ws->norm, &maxSym, &al, S, off + 1, hb, 6);
+        const uint32_t hs = fse_read_ncount(norm, &maxSym, &al, S, off + 1, hb, 6);
         if (!hs || hs >= hb) return 0;
-        // weights FSE table: symbols in ws->sym[256..], nbBits/newState packed in ws->huf[0..63]
-        uint8_t* fsym = ws->sym + 256;
+        // the weights' FSE table (at most 64 states): symbol per state, nbBits | newState << 8
+        uint8_t fsym[64]; uint16_t fdt[64];
         {
             const uint32_t size2 = 1u << al, mask = size2 - 1u; uint32_t high = size2 - 1u;
-            for (uint32_t s = 0; s <= maxSym; s++) { if (ws->norm[s] == -1) { fsym[high--] = (uint8_t)s; ws->nxt[s] = 1; } else ws->nxt[s] = (uint16_t)ws->norm[s]; }
+            for (uint32_t s = 0; s <= maxSym; s++) { if (norm[s] == -1) { fsym[high--] = (uint8_t)s; nxt[s] = 1; } else nxt[s] = (uint16_t)norm[s]; }
             const uint32_t step = (size2 >> 1) + (size2 >> 3) + 3u; uint32_t pos = 0;
             for (uint32_t s = 0; s <= maxSym; s++)
-                for (int i = 0; i < ws->norm[s]; i++) { fsym[pos] = (uint8_t)s; pos = (pos + step) & mask; while (pos > high) pos = (pos + step) & mask; }
+                for (int i = 0; i < norm[s]; i++) { fsym[pos] = (uint8_t)s; pos = (pos + step) & mask; while (pos > high) pos = (pos + step) & mask; }
             if (pos != 0) return 0;
             for (uint32_t u = 0; u < size2; u++) {
-                const uint32_t s = fsym[u], ns = ws->nxt[s]++;
+                const uint32_t s = fsym[u], ns = nxt[s]++;
                 const uint32_t nbb = al - highbit32(ns);
-                ws->huf[u] = (uint16_t)(nbb | ((((ns << nbb) - size2) & 0xFFu) << 8));     // newState < 64
+                fdt[u] = (uint16_t)(nbb | ((((ns << nbb) - size2) & 0xFFu) << 8));     // newState < 64
             }
         }
         BwdBits b; if (b.init(&S, off + 1 + hs, hb - hs)) return 0;
@@ -433,10 +415,10 @@ template <class WS> __device__ uint32_t huf_read_table(WS* ws, const Src& S, uin
         if (b.overflow) return 0;
         for (;;) {
             if (nw > 253) return 0;
-            w[nw++] = fsym[s1]; { const uint32_t e = ws->huf[s1]; s1 = (e >> 8) + b.read(e & 255u); }
+            w[nw++] = fsym[s1]; { const uint32_t e = fdt[s1]; s1 = (e >> 8) + b.read(e & 255u); }
             if (b.overflow) { w[nw++] = fsym[s2]; break; }
             if (nw > 253) return 0;
-            w[nw++] = fsym[s2]; { const uint32_t e = ws->huf[s2]; s2 = (e >> 8) + b.read(e & 255u); }
+            w[nw++] = fsym[s2]; { const uint32_t e = fdt[s2]; s2 = (e >> 8) + b.read(e & 255u); }
             if (b.overflow) { w[nw++] = fsym[s1]; break; }
         }
     }
@@ -451,18 +433,26 @@ template <class WS> __device__ uint32_t huf_read_table(WS* ws, const Src& S, uin
     w[nw++] = (uint8_t)(highbit32(rest) + 1u);
     for (uint32_t i = 0; i < nw; i++) rank[w[i]]++;
     if (rank[1] < 2 || (rank[1] & 1u)) return 0;
-    uint32_t start[13], pos = 0;
+    *nwOut = nw; *maxBitsOut = maxBits;
+    return used;
+}
+
+// Fill the 2^maxBits-entry decoding table (symbol | nbBits << 8) from checked weights: the symbols of weight r take
+// consecutive runs of 2^(r-1) entries from the weight class's start.  Thread k of n writes the entries i = k (mod n) of
+// every run.
+__device__ void huf_fill(uint16_t* huf, const uint8_t* w, uint32_t nw, uint32_t maxBits, uint32_t k, uint32_t n) {
+    uint32_t rank[13], start[13];
+    for (uint32_t r = 0; r < 13; r++) rank[r] = 0;
+    for (uint32_t i = 0; i < nw; i++) rank[w[i]]++;
+    uint32_t pos = 0;
     for (uint32_t r = 1; r <= maxBits; r++) { start[r] = pos; pos += rank[r] << (r - 1u); }
     for (uint32_t s = 0; s < nw; s++) {
         const uint32_t r = w[s]; if (!r) continue;
         const uint32_t len = 1u << (r - 1u); const uint16_t e = (uint16_t)(s | ((maxBits + 1u - r) << 8));
-        for (uint32_t i = 0; i < len; i++) ws->huf[start[r] + i] = e;
+        for (uint32_t i = k; i < len; i += n) huf[start[r] + i] = e;
         start[r] += len;
     }
-    ws->hufBits = maxBits;
-    return used;
 }
-
 // Hot-loop reader (32-bit arithmetic): `cont` holds stream bytes [bytePos, bytePos+8); the next unread bit is
 // bit (63 - consumed) of it.  After reload() consumed <= 7, so 57 bits can be read before the next reload.
 // Bytes below the stream start read as zero; left() < 0 means the stream was over-read.
@@ -482,7 +472,14 @@ struct FastBwd {
         cont = fetch();
         return 0;
     }
-    __device__ __forceinline__ void reload() { bytePos -= (int32_t)(consumed >> 3); consumed &= 7u; cont = fetch(); }
+    // The stream is read downwards: the line 256 bytes below is asked into L2 now, so that the reload that reaches it does not wait
+    // for HBM (one such wait per 128 bytes was the largest part of a stream's time).
+    __device__ __forceinline__ void reload() {
+        bytePos -= (int32_t)(consumed >> 3); consumed &= 7u; cont = fetch();
+#ifndef B2Z_CUEMU
+        if (bytePos >= 256) asm volatile("prefetch.L2 [%0];" :: "l"(S->w + ((base + (uint32_t)bytePos - 256u) >> 3)));
+#endif
+    }
     __device__ __forceinline__ uint32_t read(uint32_t n) {                      // n <= 32 (0 allowed)
         const uint32_t v = (uint32_t)(((cont << consumed) >> 1) >> (63u - n));
         consumed += n;
@@ -491,180 +488,127 @@ struct FastBwd {
     __device__ __forceinline__ int32_t left() const { return bytePos * 8 + 64 - (int32_t)consumed; }   // unread bits
 };
 
-// one Huffman stream, one lane
-template <class WS> __device__ bool huf_decode_stream(const WS* ws, const Src& S, uint64_t off, uint32_t size, uint8_t* dst, uint32_t n) {
-    FastBwd b; if (b.init(&S, off, size)) return false;
-    const uint32_t mb = ws->hufBits;
-    for (uint32_t i = 0; i < n; i++) {
-        if (b.consumed > 64u - 11u) b.reload();
-        const uint32_t e = ws->huf[(uint32_t)((b.cont << b.consumed) >> (64u - mb))];
-        dst[i] = (uint8_t)e; b.consumed += (e >> 8);
-    }
-    return b.left() == 0;
-}
-
 // ---------------------------------------------------------------- D1: entropy decode
+// Four kernels, two per section, and no table ever leaves the SM:
+//   zstd_dec_entropy_kernel<0>  (warp / block)    literal headers; raw / RLE literals are expanded here
+//   zstd_dec_lit_streams_kernel (4 threads / block) builds the Huffman table in shared memory, one thread per stream decodes
+//   zstd_dec_entropy_kernel<1>  (thread / block)  sequence headers: where the three table descriptions are (an earlier block's
+//                                                 for repeat mode), their sizes checked; the bookkeeping of blocks without sequences
+//   zstd_dec_seq_streams_kernel (thread / block)  builds the three FSE tables in shared memory and decodes the bitstream
+// Each serial bitstream is decoded by ONE THREAD, so that thousands of dependent chains overlap.  A table is built from the
+// description in src (an earlier block's for treeless literals and repeat mode: any block may be read, a CTA depends on no other
+// CTA).  The stream kernels loop over their groups of blocks, so they do not depend on the grid they are given.
 #define SEQ_PACK(ob, ll, ml) ((uint64_t)(ob) | ((uint64_t)(ll) << 30) | ((uint64_t)((ml) - 3u) << 47))
 
-// Table stage, one warp per compressed block.  ROLE 0: raw/RLE literals are expanded here, for Huffman literals the
-// decoding table is built (lane 0) and spilled to global scratch; ROLE 1: the three FSE tables of the sequences
-// section are built and spilled.  The serial bitstreams themselves are decoded by the *_streams kernels below with
-// ONE THREAD PER STREAM, so that thousands of dependent chains overlap instead of one per warp.
-struct LitJob { uint64_t off; uint32_t size, regen, streams, hufBits; };
-struct SeqJob { uint64_t bsOff; uint32_t bsLeft, nbSeq, litRegen, logs; };
+typedef uint16_t SeqEnt;                            // one state of a sequence decoding table (B2Z_SEQ_TAB layout above)
+struct LitJob { uint64_t off; uint32_t size, regen, streams, type; };          // Huffman literals: the section after its header
+struct SeqJob { uint64_t bsOff, desc[3]; uint32_t bsLeft, nbSeq, litRegen, modes, avail[3], pad; };  // table t: description, mode, bytes left
 #define D1_WARPS(ROLE) ((ROLE) == 0 ? 6 : 4)
+// The table arguments (hufTabs, seqTabs) are not used: the tables are built where they are read.
 template <int ROLE> __global__ void __launch_bounds__(D1_WARPS(ROLE) * 32)
 zstd_dec_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, DecBlock* __restrict__ blocks, uint32_t nBlocks,
                         uint8_t* __restrict__ lits, uint16_t* __restrict__ hufTabs, LitJob* __restrict__ litJobs,
                         SeqEnt* __restrict__ seqTabs, SeqJob* __restrict__ seqJobs) {
-    typedef DecWST<ROLE> DecWS;
-    __shared__ DecWS wsAll[D1_WARPS(ROLE)];
-    const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
-    DecWS* ws = &wsAll[wib];
     Src S; S.w = reinterpret_cast<const uint64_t*>(src); S.nWords = (srcSize + 7) >> 3; S.size = srcSize;
-    for (uint32_t bi = blockIdx.x * D1_WARPS(ROLE) + wib; bi < nBlocks; bi += gridDim.x * D1_WARPS(ROLE)) {
+    if (ROLE == 0) {
+        const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
+        for (uint32_t bi = blockIdx.x * D1_WARPS(0) + wib; bi < nBlocks; bi += gridDim.x * D1_WARPS(0)) {
+            const DecBlock blk = blocks[bi];
+            if (blk.type != 2) continue;
+            const LitHdr lh = parse_lit_hdr(S, blk.srcOff, blk.cSize);
+            uint8_t* lit = lits + (size_t)blk.slot * 131072u;
+            if (lh.type == 0) { for (uint32_t i = lane; i < lh.regen; i += 32) lit[i] = (uint8_t)S.u8(blk.srcOff + lh.hdr + i); }
+            else if (lh.type == 1) { const uint8_t v = (uint8_t)S.u8(blk.srcOff + lh.hdr); for (uint32_t i = lane; i < lh.regen; i += 32) lit[i] = v; }
+            if (lane == 0) { LitJob j; j.off = blk.srcOff + lh.hdr; j.size = lh.csize; j.regen = lh.regen; j.streams = lh.type >= 2 ? lh.streams : 0u; j.type = lh.type; litJobs[bi] = j; }
+        }
+        return;
+    }
+    const uint32_t maxSymT[3] = { 35, 31, 52 }, maxLogT[3] = { 9, 8, 9 };
+    for (uint32_t bi = blockIdx.x * blockDim.x + threadIdx.x; bi < nBlocks; bi += gridDim.x * blockDim.x) {
         const DecBlock blk = blocks[bi];
         if (blk.type != 2) continue;
         uint32_t err = 0;
         const LitHdr lh = parse_lit_hdr(S, blk.srcOff, blk.cSize);
-        uint8_t* lit = lits + (size_t)blk.slot * 131072u;
-        // ---- literals
-        if (ROLE == 0) {
-        if (lh.type == 0) { for (uint32_t i = lane; i < lh.regen; i += 32) lit[i] = (uint8_t)S.u8(blk.srcOff + lh.hdr + i); }
-        else if (lh.type == 1) { const uint8_t v = (uint8_t)S.u8(blk.srcOff + lh.hdr); for (uint32_t i = lane; i < lh.regen; i += 32) lit[i] = v; }
-        else {
-            uint32_t tdesc = 0;                                  // this block's own table description bytes
-            if (lane == 0) {
-                const DecBlock sb = blocks[blk.hufSrc];
-                const LitHdr sh = parse_lit_hdr(S, sb.srcOff, sb.cSize);
-                const uint32_t u = (sh.ok && sh.type == 2) ? huf_read_table(ws, S, sb.srcOff + sh.hdr, sh.csize) : 0u;
-                if (!u) err = B2Z_DERR_CORRUPT;
-                if (lh.type == 2) tdesc = u;
+        const uint32_t so = lh.hdr + lh.csize;
+        const SeqHdr sh = parse_seq_hdr(S, blk.srcOff + so, blk.cSize - so);
+        const uint32_t nbSeq = sh.nbSeq;
+        if (nbSeq > B2Z_DEC_MAXSEQ) err = B2Z_DERR_CORRUPT;
+        SeqJob job; job.bsOff = 0; job.bsLeft = 0; job.nbSeq = 0; job.litRegen = lh.regen; job.modes = 0; job.pad = 0;
+        for (int t = 0; t < 3; t++) { job.desc[t] = 0; job.avail[t] = 0; }
+        if (nbSeq && !err) {
+            uint64_t bsOff = blk.srcOff + so + sh.hdr; uint32_t bsLeft = blk.cSize - so - sh.hdr;
+            int16_t norm[56];
+            for (int t = 0; t < 3 && !err; t++) {
+                uint64_t d; uint32_t mode, avail;
+                const uint32_t ownMode = (sh.modes >> (6 - 2 * t)) & 3u;
+                if (ownMode == 3) {
+                    if (!locate_seq_table(S, blocks[blk.tblSrc[t]], t, norm, &d, &mode, &avail) || mode == 3) { err = B2Z_DERR_CORRUPT; break; }
+                } else { d = bsOff; mode = ownMode; avail = bsLeft; }
+                uint32_t used = 0;
+                if (mode == 1) { if (avail < 1 || S.u8(d) > maxSymT[t]) err = B2Z_DERR_CORRUPT; else used = 1; }
+                else if (mode == 2) { uint32_t ms = maxSymT[t], lg; used = fse_read_ncount(norm, &ms, &lg, S, d, avail, maxLogT[t]); if (!used) err = B2Z_DERR_CORRUPT; }
+                job.desc[t] = d; job.avail[t] = avail; job.modes |= mode << (2 * t);
+                if (ownMode != 3) { if (used > bsLeft) err = B2Z_DERR_CORRUPT; else { bsOff += used; bsLeft -= used; } }
             }
-            err = __shfl_sync(B2Z_FULL, err, 0); tdesc = __shfl_sync(B2Z_FULL, tdesc, 0);
-            __syncwarp();
-            if (!err) {
-                // spill the decoding table; the streams are decoded by zstd_dec_lit_streams_kernel (one thread per stream)
-                uint16_t* gt = hufTabs + (size_t)bi * 2048u;
-                const uint32_t nEnt = 1u << ws->hufBits;
-                for (uint32_t i = lane; i < nEnt; i += 32) gt[i] = ws->huf[i];
-                if (lane == 0) { LitJob j; j.off = blk.srcOff + lh.hdr + tdesc; j.size = tdesc <= lh.csize ? lh.csize - tdesc : 0xFFFFFFFFu; j.regen = lh.regen; j.streams = lh.streams; j.hufBits = ws->hufBits; litJobs[bi] = j; }
-            }
+            if (!err) { job.bsOff = bsOff; job.bsLeft = bsLeft; job.nbSeq = nbSeq; }
         }
-        if (lane == 0 && (err || lh.type < 2)) { LitJob j; j.off = 0; j.size = 0; j.regen = 0; j.streams = 0; j.hufBits = 0; litJobs[bi] = j; }
-        if (lane == 0 && err) atomicOr(&blocks[bi].status, err);
-        }
-        __syncwarp();
-        // ---- sequences (lane 0)
-        uint32_t nbSeq = 0;
-        if (ROLE == 1) {
-        SeqJob job; job.bsOff = 0; job.bsLeft = 0; job.nbSeq = 0; job.litRegen = lh.regen; job.logs = 0;
-        if (lane == 0 && !err) {
-            const uint32_t so = lh.hdr + lh.csize;
-            const SeqHdr sh = parse_seq_hdr(S, blk.srcOff + so, blk.cSize - so);
-            nbSeq = sh.nbSeq;
-            if (nbSeq > B2Z_DEC_MAXSEQ) err = B2Z_DERR_CORRUPT;
-            if (nbSeq && !err) {
-                const uint32_t maxSymT[3] = { 35, 31, 52 }, maxLogT[3] = { 9, 8, 9 }, defMax[3] = { 35, 28, 52 }, defLog[3] = { 6, 5, 6 };
-                uint64_t bsOff = blk.srcOff + so + sh.hdr; uint32_t bsLeft = blk.cSize - so - sh.hdr;
-                for (int t = 0; t < 3 && !err; t++) {
-                    uint64_t d; uint32_t mode, avail;
-                    const uint32_t ownMode = (sh.modes >> (6 - 2 * t)) & 3u;
-                    if (ownMode == 3) {
-                        if (!locate_seq_table(S, blocks[blk.tblSrc[t]], t, ws, &d, &mode, &avail) || mode == 3) { err = B2Z_DERR_CORRUPT; break; }
-                    } else { d = bsOff; mode = ownMode; avail = bsLeft; }
-                    uint32_t used = 0;
-                    if (mode == 0) {
-                        const int16_t* dn = t == 0 ? k_LL_defNorm : (t == 1 ? k_OF_defNorm : k_ML_defNorm);
-                        for (uint32_t s = 0; s <= defMax[t]; s++) ws->norm[s] = dn[s];
-                        if (!build_seq_table(ws, t, ws->norm, defMax[t], defLog[t])) err = B2Z_DERR_CORRUPT;
-                    } else if (mode == 1) {
-                        const uint32_t s = S.u8(d);
-                        if (avail < 1 || s > maxSymT[t]) err = B2Z_DERR_CORRUPT;
-                        else {
-                            SeqEnt e; e.nbBits = 0; e.next = 0;
-                            if (t == 0) { e.base = k_LL_base[s]; e.nbAdd = k_LL_bits[s]; } else if (t == 2) { e.base = k_ML_base[s]; e.nbAdd = k_ML_bits[s]; } else { e.base = 1u << s; e.nbAdd = (uint8_t)s; }
-                            ws->tab(t)[0] = e; ws->tabLog[t] = 0; used = 1;
-                        }
-                    } else {
-                        uint32_t ms = maxSymT[t], lg;
-                        used = fse_read_ncount(ws->norm, &ms, &lg, S, d, avail, maxLogT[t]);
-                        if (!used || !build_seq_table(ws, t, ws->norm, ms, lg)) err = B2Z_DERR_CORRUPT;
-                    }
-                    if (ownMode != 3) { if (used > bsLeft) err = B2Z_DERR_CORRUPT; else { bsOff += used; bsLeft -= used; } }
-                }
-                if (!err) { job.bsOff = bsOff; job.bsLeft = bsLeft; job.nbSeq = nbSeq; job.litRegen = lh.regen; job.logs = ws->tabLog[0] | (ws->tabLog[1] << 8) | (ws->tabLog[2] << 16); }
-            }
-        }
-        err = __shfl_sync(B2Z_FULL, err, 0); nbSeq = __shfl_sync(B2Z_FULL, nbSeq, 0);
-        __syncwarp();                                                 // lane 0's tables are visible to the warp
-        if (!err && nbSeq) {                                          // spill the three tables (LL 512 | OF 256 | ML 512 entries)
-            uint2* gt = reinterpret_cast<uint2*>(seqTabs + (size_t)bi * 1280u);
-            const uint2* st2 = reinterpret_cast<const uint2*>(ws->tabs);
-            const uint32_t nL = 1u << ws->tabLog[0], nO = 1u << ws->tabLog[1], nM = 1u << ws->tabLog[2];
-            for (uint32_t i = lane; i < nL; i += 32) gt[i] = st2[i];
-            for (uint32_t i = lane; i < nO; i += 32) gt[512 + i] = st2[512 + i];
-            for (uint32_t i = lane; i < nM; i += 32) gt[768 + i] = st2[768 + i];
-        }
-        if (lane == 0) {
-            if (err) { job.nbSeq = 0; job.bsLeft = 0; }
-            if (!nbSeq && !err) { job.bsOff = 0; job.bsLeft = 0; job.nbSeq = 0; job.litRegen = lh.regen; job.logs = 0; }
-            seqJobs[bi] = job;
-            blocks[bi].regen = (err || nbSeq) ? 0u : lh.regen; blocks[bi].nbSeq = 0; blocks[bi].litSize = lh.regen; if (err) atomicOr(&blocks[bi].status, err);
-        }
-        }
-        __syncwarp();
+        seqJobs[bi] = job;
+        blocks[bi].regen = (err || nbSeq) ? 0u : lh.regen; blocks[bi].nbSeq = 0; blocks[bi].litSize = lh.regen;
+        if (err) atomicOr(&blocks[bi].status, err);
     }
 }
 
-// ---------------------------------------------------------------- D1b: one thread per stream
-// Literal streams.  The decoding tables (up to 4 KiB per block, 128 MB for the 32 768 blocks of 4 GiB) do not fit L2 while every stream
-// of the input is in flight, and a look-up per symbol from HBM was what this kernel waited for.  A CTA therefore
-// serves LIT_BLOCKS blocks (4 streams each) and first copies their tables into shared memory: the per-symbol chain is then two shifts,
-// one shared-memory load and an add.
+// Literal streams: B2Z_LIT_BLOCKS blocks per CTA, 4 threads per block (one per Huffman stream).  Thread 0 of a block decodes the
+// weights, the block's 4 threads fill its 4 KiB table and decode.
 #define B2Z_LIT_BLOCKS 16u
 __global__ void __launch_bounds__(B2Z_LIT_BLOCKS * 4u)
 zstd_dec_lit_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, DecBlock* __restrict__ blocks, uint32_t nBlocks,
                             uint8_t* __restrict__ lits, const uint16_t* __restrict__ hufTabs, const LitJob* __restrict__ litJobs) {
-    B2Z_EXTERN_SMEM(uint16_t, smTab);                                   // [B2Z_LIT_BLOCKS][2048]
-    const uint32_t b0 = blockIdx.x * B2Z_LIT_BLOCKS;
-    {   // stage the tables of this CTA's blocks (16-byte copies; a block without Huffman streams has none)
-        const uint4* g4 = reinterpret_cast<const uint4*>(hufTabs + (size_t)b0 * 2048u);
-        uint4* s4 = reinterpret_cast<uint4*>(smTab);
-        for (uint32_t i = threadIdx.x; i < B2Z_LIT_BLOCKS * 256u; i += B2Z_LIT_BLOCKS * 4u) {
-            const uint32_t bb = b0 + (i >> 8);
-            if (bb < nBlocks && blocks[bb].type == 2) {                  // (raw / RLE blocks have no job record: nothing was written there)
-                const LitJob jj = litJobs[bb];
-                if (jj.streams && (i & 255u) < ((1u << jj.hufBits) + 7u) / 8u) s4[i] = __ldg(g4 + i);
-            }
-        }
-    }
-    __syncthreads();
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    const uint32_t bi = t >> 2, k = t & 3u;
-    if (bi >= nBlocks) return;
-    const LitJob j = litJobs[bi];
-    if (!j.streams || blocks[bi].type != 2) return;
+    B2Z_EXTERN_SMEM(uint16_t, smTab);                                   // [B2Z_LIT_BLOCKS][2048] decoding tables
+    __shared__ uint8_t smW[B2Z_LIT_BLOCKS][256];                        // their weights
+    const uint32_t j = threadIdx.x >> 2, k = threadIdx.x & 3u, bi = blockIdx.x * B2Z_LIT_BLOCKS + j;
+    const uint32_t lead = (threadIdx.x & 31u) & ~3u;                    // lane of the block's thread 0
+    uint16_t* tab = smTab + (size_t)j * 2048u;
     Src S; S.w = reinterpret_cast<const uint64_t*>(src); S.nWords = (srcSize + 7) >> 3; S.size = srcSize;
+    LitJob lj; lj.off = 0; lj.size = 0; lj.regen = 0; lj.streams = 0; lj.type = 0;
+    if (bi < nBlocks && blocks[bi].type == 2) lj = litJobs[bi];         // (raw / RLE blocks have no job record)
+    // ---- the table: weights (thread 0 of the block), then the fill (the block's 4 threads)
+    uint32_t tdesc = 0, nw = 0, maxBits = 0, err = 0;
+    if (lj.streams && k == 0) {
+        const DecBlock sb = blocks[blocks[bi].hufSrc];
+        const LitHdr sh = parse_lit_hdr(S, sb.srcOff, sb.cSize);
+        const uint32_t u = (sh.ok && sh.type == 2) ? huf_read_weights(smW[j], &nw, &maxBits, S, sb.srcOff + sh.hdr, sh.csize) : 0u;
+        if (!u) err = B2Z_DERR_CORRUPT;
+        if (lj.type == 2) tdesc = u;
+    }
+    err = __shfl_sync(B2Z_FULL, err, lead); tdesc = __shfl_sync(B2Z_FULL, tdesc, lead);
+    nw = __shfl_sync(B2Z_FULL, nw, lead); maxBits = __shfl_sync(B2Z_FULL, maxBits, lead);
+    __syncwarp();                                                       // the weights are visible to the block's threads
+    if (lj.streams && !err) huf_fill(tab, smW[j], nw, maxBits, k, 4u);
+    __syncwarp();                                                       // the table is complete
+    if (!lj.streams) return;
+    if (err) { if (k == 0) atomicOr(&blocks[bi].status, err); return; }
+    // ---- the streams: one thread each
     uint8_t* lit = lits + (size_t)blocks[bi].slot * 131072u;
-    const uint16_t* tab = smTab + (size_t)(bi - b0) * 2048u;
+    const uint64_t jOff = lj.off + tdesc;
+    const uint32_t jSize = tdesc <= lj.size ? lj.size - tdesc : 0xFFFFFFFFu;
     bool ok = true;
     uint64_t off = 0; uint32_t size = 0, cnt = 0; uint8_t* dst = lit;
-    if (j.size == 0xFFFFFFFFu) ok = false;
-    else if (j.streams == 1) { if (k) return; off = j.off; size = j.size; cnt = j.regen; }
+    if (jSize == 0xFFFFFFFFu) ok = false;
+    else if (lj.streams == 1) { if (k) return; off = jOff; size = jSize; cnt = lj.regen; }
     else {
-        if (j.size < 6) ok = false;
+        if (jSize < 6) ok = false;
         else {
-            const uint64_t jt = S.le64(j.off);
+            const uint64_t jt = S.le64(jOff);
             const uint32_t s1 = (uint32_t)jt & 0xFFFFu, s2 = (uint32_t)(jt >> 16) & 0xFFFFu, s3 = (uint32_t)(jt >> 32) & 0xFFFFu;
-            const uint32_t seg = (j.regen + 3u) / 4u;
-            if (6u + s1 + s2 + s3 > j.size || seg * 3u > j.regen) ok = false;
+            const uint32_t seg = (lj.regen + 3u) / 4u;
+            if (6u + s1 + s2 + s3 > jSize || seg * 3u > lj.regen) ok = false;
             else {
-                const uint32_t s4 = j.size - 6u - s1 - s2 - s3;
+                const uint32_t s4 = jSize - 6u - s1 - s2 - s3;
                 const uint32_t so = k == 0 ? 0u : (k == 1 ? s1 : (k == 2 ? s1 + s2 : s1 + s2 + s3));
                 size = k == 0 ? s1 : (k == 1 ? s2 : (k == 2 ? s3 : s4));
-                cnt = k < 3 ? seg : j.regen - 3u * seg;
-                off = j.off + 6u + so; dst = lit + k * seg;
+                cnt = k < 3 ? seg : lj.regen - 3u * seg;
+                off = jOff + 6u + so; dst = lit + k * seg;
             }
         }
     }
@@ -672,8 +616,8 @@ zstd_dec_lit_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
         FastBwd b;
         if (b.init(&S, off, size)) ok = false;
         else {
-            const uint32_t mb = j.hufBits;
-            // symbols are gathered eight at a time and stored as one aligned word (head and tail byte by byte): every lane writes its own stream
+            const uint32_t mb = maxBits;
+            // symbols are gathered eight at a time and stored as one aligned word (head and tail byte by byte): every thread writes its own stream
             uint32_t i = 0;
             const uint32_t head = (uint32_t)((8u - ((uintptr_t)dst & 7u)) & 7u);
             for (; i < cnt && i < head; i++) {
@@ -702,60 +646,99 @@ zstd_dec_lit_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
     if (!ok) atomicOr(&blocks[bi].status, B2Z_DERR_CORRUPT);
 }
 
+// Sequence streams: groups of B2Z_SEQ_BLOCKS blocks, one thread per block (the CTA's other threads leave).  The thread builds its
+// block's three tables in its 2.5 KiB of shared memory (about 1 % of the block's decode on text) and decodes the bitstream from
+// them: the chain of a sequence is shared-memory loads and bit arithmetic, with no global round trip.  17 x 2560 bytes + the symbol
+// table are 43.9 KB per CTA: five CTAs (85 chains) per SM of 228 KB, so 32 768 blocks take three waves on 132 SMs.
+#define B2Z_SEQ_BLOCKS 17u
 __global__ void __launch_bounds__(128)
 zstd_dec_seq_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, DecBlock* __restrict__ blocks, uint32_t nBlocks,
                             uint64_t* __restrict__ seqs, const SeqEnt* __restrict__ seqTabs, const SeqJob* __restrict__ seqJobs) {
-    const uint32_t bi = blockIdx.x * blockDim.x + threadIdx.x;
-    if (bi >= nBlocks || blocks[bi].type != 2) return;
-    const SeqJob j = seqJobs[bi];
-    if (!j.nbSeq) return;
+    __shared__ uint32_t k_seqSym[89];                                   // LL symbols [0,36) | ML symbols [36,89): baseline | extra bits << 24
+    __shared__ SeqEnt smTab[B2Z_SEQ_BLOCKS][B2Z_SEQ_TAB];
+    for (uint32_t i = threadIdx.x; i < 89u; i += blockDim.x) k_seqSym[i] = i < 36u ? k_LL_base[i] | ((uint32_t)k_LL_bits[i] << 24) : k_ML_base[i - 36u] | ((uint32_t)k_ML_bits[i - 36u] << 24);
+    __syncthreads();
+    if (threadIdx.x >= B2Z_SEQ_BLOCKS) return;
+    SeqEnt* tab = smTab[threadIdx.x];
     Src S; S.w = reinterpret_cast<const uint64_t*>(src); S.nWords = (srcSize + 7) >> 3; S.size = srcSize;
-    const uint2* __restrict__ tab = reinterpret_cast<const uint2*>(seqTabs + (size_t)bi * 1280u);
-    uint32_t err = 0, regen = 0;
-    FastBwd b;
-    if (b.init(&S, j.bsOff, j.bsLeft)) err = B2Z_DERR_CORRUPT;
-    else {
-        uint32_t sL = b.read(j.logs & 255u), sO = b.read((j.logs >> 8) & 255u), sM = b.read((j.logs >> 16) & 255u);   // <= 26 bits
-        if (b.left() < 0) err = B2Z_DERR_CORRUPT;
-        uint64_t* out = seqs + (size_t)blocks[bi].slot * B2Z_DEC_MAXSEQ;
-        uint32_t litUsed = 0, total = 0, near = 0;
-        // the repcode history as a function of the history before the block (b2z_dec.h DecBlock::repX): slot = value (sym 0) or
-        // (initial slot sym - 1) minus value.  ZSTD_decodeSequence's update rules, zstd_decompress_block.c:1290-1312
-        uint32_t v0 = 0, v1 = 0, v2 = 0, y0 = 1, y1 = 2, y2 = 3;
-        for (uint32_t i = 0; i < j.nbSeq && !err; i++) {
-            const uint2 rL = __ldg(tab + sL), rO = __ldg(tab + 512u + sO), rM = __ldg(tab + 768u + sM);     // {base, nbAdd | nbBits<<8 | next<<16}
-            const uint32_t aL = rL.y & 255u, aO = rO.y & 255u, aM = rM.y & 255u;
-            if (aO > 30u) { err = B2Z_DERR_UNSUPPORTED; break; }
-            b.reload();
-            const uint32_t ob = rO.x + b.read(aO);
-            if (aO + aM + aL > 56u) b.reload();
-            const uint32_t ml = rM.x + b.read(aM);
-            const uint32_t ll = rL.x + b.read(aL);
-            if (i + 1 < j.nbSeq) {
-                if (aO + aM + aL > 30u) b.reload();                                                     // + <= 26 state bits
-                sL = (rL.y >> 16) + b.read((rL.y >> 8) & 255u); sM = (rM.y >> 16) + b.read((rM.y >> 8) & 255u); sO = (rO.y >> 16) + b.read((rO.y >> 8) & 255u);
-            }
-            litUsed += ll; total += ll + ml;
-            if (b.left() < 0 || litUsed > j.litRegen || total > 131072u || ob >= (1u << 30)) { err = B2Z_DERR_CORRUPT; break; }
-            out[i] = SEQ_PACK(ob, ll, ml);
-            // a source at most one unit's span before the block: the block's unit cannot run beside the unit before it (stage D2 counts these)
-            near |= (uint32_t)(ob > 3u && ob - 3u > total - ml && ob - 3u - (total - ml) <= B2Z_DEC_UNIT_BLOCKS * 131072u);
-            if (ob > 3u) { v2 = v1; y2 = y1; v1 = v0; y1 = y0; v0 = ob - 3u; y0 = 0u; }
-            else {
-                const uint32_t idx = ob - 1u + (ll == 0u);
-                if (idx == 1u) { const uint32_t tv = v0, ty = y0; v0 = v1; y0 = y1; v1 = tv; y1 = ty; }
-                else if (idx == 2u) { const uint32_t tv = v2, ty = y2; v2 = v1; y2 = y1; v1 = v0; y1 = y0; v0 = tv; y0 = ty; }
-                else if (idx == 3u) { v2 = v1; y2 = y1; v1 = v0; y1 = y0; v0 = y0 ? v0 + 1u : v0 - 1u; }      // rep0 - 1: one more to subtract, or a smaller value
+    for (uint32_t g = blockIdx.x; (uint64_t)g * B2Z_SEQ_BLOCKS < nBlocks; g += gridDim.x) {
+        const uint32_t bi = g * B2Z_SEQ_BLOCKS + threadIdx.x;
+        if (bi >= nBlocks) break;
+        if (blocks[bi].type != 2) continue;
+        const SeqJob j = seqJobs[bi];
+        if (!j.nbSeq) continue;
+        uint32_t err = 0, logs[3] = { 0, 0, 0 };
+        {
+            const uint32_t maxSymT[3] = { 35, 31, 52 }, maxLogT[3] = { 9, 8, 9 }, defMax[3] = { 35, 28, 52 }, defLog[3] = { 6, 5, 6 };
+            int16_t norm[56];
+            for (int t = 0; t < 3 && !err; t++) {
+                const uint32_t mode = (j.modes >> (2 * t)) & 3u;
+                if (mode == 0) {
+                    const int16_t* dn = t == 0 ? k_LL_defNorm : (t == 1 ? k_OF_defNorm : k_ML_defNorm);
+                    for (uint32_t s = 0; s <= defMax[t]; s++) norm[s] = dn[s];
+                    if (!build_seq_table(tab + seq_tab_off(t), norm, defMax[t], defLog[t])) err = B2Z_DERR_CORRUPT;
+                    logs[t] = defLog[t];
+                } else if (mode == 1) {
+                    tab[seq_tab_off(t)] = (SeqEnt)(S.u8(j.desc[t]) | (1u << 6)); logs[t] = 0;         // one state: no bits, next state 0
+                } else {
+                    uint32_t ms = maxSymT[t], lg;
+                    if (!fse_read_ncount(norm, &ms, &lg, S, j.desc[t], j.avail[t], maxLogT[t]) || !build_seq_table(tab + seq_tab_off(t), norm, ms, lg)) err = B2Z_DERR_CORRUPT;
+                    logs[t] = lg;
+                }
             }
         }
-        blocks[bi].repX[0] = v0; blocks[bi].repX[1] = v1; blocks[bi].repX[2] = v2; blocks[bi].repSym = y0 | (y1 << 2) | (y2 << 4);
-        blocks[bi].nearBehind = near;
-        if (!err && b.left() != 0) err = B2Z_DERR_CORRUPT;
-        regen = total + (j.litRegen - litUsed);
-        if (regen > 131072u) err = B2Z_DERR_CORRUPT;
+        uint32_t regen = 0;
+        FastBwd b;
+        if (err || b.init(&S, j.bsOff, j.bsLeft)) err = B2Z_DERR_CORRUPT;
+        else {
+            const SeqEnt* tL = tab; const SeqEnt* tO = tab + 512; const SeqEnt* tM = tab + 768;
+            const uint32_t gL = logs[0], gO = logs[1], gM = logs[2];
+            uint32_t sL = b.read(gL), sO = b.read(gO), sM = b.read(gM);                               // <= 26 bits
+            if (b.left() < 0) err = B2Z_DERR_CORRUPT;
+            uint64_t* out = seqs + (size_t)blocks[bi].slot * B2Z_DEC_MAXSEQ;
+            uint32_t litUsed = 0, total = 0, near = 0;
+            // the repcode history as a function of the history before the block (b2z_dec.h DecBlock::repX): slot = value (sym 0) or
+            // (initial slot sym - 1) minus value.  ZSTD_decodeSequence's update rules, zstd_decompress_block.c:1290-1312
+            uint32_t v0 = 0, v1 = 0, v2 = 0, y0 = 1, y1 = 2, y2 = 3;
+            for (uint32_t i = 0; i < j.nbSeq && !err; i++) {
+                const uint32_t eL = tL[sL], eO = tO[sO], eM = tM[sM];                                 // symbol | ns << 6
+                const uint32_t aO = eO & 63u;
+                if (aO > 30u) { err = B2Z_DERR_UNSUPPORTED; break; }
+                const uint32_t xL = k_seqSym[eL & 63u], xM = k_seqSym[36u + (eM & 63u)];
+                const uint32_t aL = xL >> 24, aM = xM >> 24;
+                b.reload();
+                const uint32_t ob = (1u << aO) + b.read(aO);
+                if (aO + aM + aL > 56u) b.reload();
+                const uint32_t ml = (xM & 0xFFFFFFu) + b.read(aM);
+                const uint32_t ll = (xL & 0xFFFFFFu) + b.read(aL);
+                if (i + 1 < j.nbSeq) {
+                    if (aO + aM + aL > 30u) b.reload();                                                 // + <= 26 state bits
+                    const uint32_t nL = eL >> 6, nM = eM >> 6, nO = eO >> 6;
+                    const uint32_t bL = gL - highbit32(nL), bM = gM - highbit32(nM), bO = gO - highbit32(nO);
+                    sL = ((nL << bL) - (1u << gL)) + b.read(bL); sM = ((nM << bM) - (1u << gM)) + b.read(bM); sO = ((nO << bO) - (1u << gO)) + b.read(bO);
+                }
+                litUsed += ll; total += ll + ml;
+                if (b.left() < 0 || litUsed > j.litRegen || total > 131072u || ob >= (1u << 30)) { err = B2Z_DERR_CORRUPT; break; }
+                out[i] = SEQ_PACK(ob, ll, ml);
+                // a source at most one unit's span before the block: the block's unit cannot run beside the unit before it (stage D2 counts these)
+                near |= (uint32_t)(ob > 3u && ob - 3u > total - ml && ob - 3u - (total - ml) <= B2Z_DEC_UNIT_BLOCKS * 131072u);
+                if (ob > 3u) { v2 = v1; y2 = y1; v1 = v0; y1 = y0; v0 = ob - 3u; y0 = 0u; }
+                else {
+                    const uint32_t idx = ob - 1u + (ll == 0u);
+                    if (idx == 1u) { const uint32_t tv = v0, ty = y0; v0 = v1; y0 = y1; v1 = tv; y1 = ty; }
+                    else if (idx == 2u) { const uint32_t tv = v2, ty = y2; v2 = v1; y2 = y1; v1 = v0; y1 = y0; v0 = tv; y0 = ty; }
+                    else if (idx == 3u) { v2 = v1; y2 = y1; v1 = v0; y1 = y0; v0 = y0 ? v0 + 1u : v0 - 1u; }      // rep0 - 1: one more to subtract, or a smaller value
+                }
+            }
+            blocks[bi].repX[0] = v0; blocks[bi].repX[1] = v1; blocks[bi].repX[2] = v2; blocks[bi].repSym = y0 | (y1 << 2) | (y2 << 4);
+            blocks[bi].nearBehind = near;
+            if (!err && b.left() != 0) err = B2Z_DERR_CORRUPT;
+            regen = total + (j.litRegen - litUsed);
+            if (regen > 131072u) err = B2Z_DERR_CORRUPT;
+        }
+        blocks[bi].regen = err ? 0u : regen; blocks[bi].nbSeq = err ? 0u : j.nbSeq;
+        if (err) atomicOr(&blocks[bi].status, err);
     }
-    blocks[bi].regen = err ? 0u : regen; blocks[bi].nbSeq = err ? 0u : j.nbSeq;
-    if (err) atomicOr(&blocks[bi].status, err);
 }
 
 // ---------------------------------------------------------------- D2: layout
@@ -1212,28 +1195,26 @@ void launch_zstd_dec_index_blocks(const uint8_t* src, uint64_t srcSize, DecFrame
 void launch_zstd_dec_entropy(const uint8_t* src, uint64_t srcSize, DecBlock* blocks, uint32_t nBlocks, uint8_t* lits, uint64_t* seqs,
                              void* scratch, uint32_t smCount, cudaStream_t st, cudaStream_t stLit, cudaEvent_t evFork, cudaEvent_t evJoin) {
     if (!nBlocks) return;
-    // scratch layout: hufTabs [nBlocks][2048] u16 | seqTabs [nBlocks][1280] SeqEnt | litJobs | seqJobs
-    uint8_t* p = (uint8_t*)scratch;
-    uint16_t* hufTabs = (uint16_t*)p; p += (size_t)nBlocks * 4096u;
-    SeqEnt* seqTabs = (SeqEnt*)p; p += (size_t)nBlocks * 1280u * sizeof(SeqEnt);
-    LitJob* litJobs = (LitJob*)p; p += (size_t)nBlocks * sizeof(LitJob);
-    SeqJob* seqJobs = (SeqJob*)p;
+    // scratch layout: litJobs [nBlocks] | seqJobs [nBlocks]; the tables themselves never leave shared memory
+    LitJob* litJobs = (LitJob*)scratch;
+    SeqJob* seqJobs = (SeqJob*)((uint8_t*)scratch + (size_t)nBlocks * sizeof(LitJob));
     // The literal and the sequence kernels only read src/blocks and write disjoint outputs, so they may run on two streams
-    // (stLit != st).  The four kernels each fill the GPU, and co-scheduling them
-    // only makes them evict each other's lines (two streams measured slower than one).
-    // The host dispatcher therefore passes stLit == st.
+    // (stLit != st).  The stream kernels each fill the GPU's shared memory, so co-scheduling them gains nothing;
+    // the host dispatcher passes stLit == st.
     if (stLit != st) { cudaEventRecord(evFork, st); cudaStreamWaitEvent(stLit, evFork, 0); }
     const uint32_t cap = smCount * 16u;
     { uint32_t grid = (nBlocks + D1_WARPS(0) - 1) / D1_WARPS(0); if (grid > cap) grid = cap;
-      zstd_dec_entropy_kernel<0><<<grid, D1_WARPS(0) * 32, 0, stLit>>>(src, srcSize, blocks, nBlocks, lits, hufTabs, litJobs, seqTabs, seqJobs);
+      zstd_dec_entropy_kernel<0><<<grid, D1_WARPS(0) * 32, 0, stLit>>>(src, srcSize, blocks, nBlocks, lits, nullptr, litJobs, nullptr, seqJobs);
       cudaFuncSetAttribute(zstd_dec_lit_streams_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(B2Z_LIT_BLOCKS * 4096u));
-      zstd_dec_lit_streams_kernel<<<(nBlocks + B2Z_LIT_BLOCKS - 1u) / B2Z_LIT_BLOCKS, B2Z_LIT_BLOCKS * 4u, B2Z_LIT_BLOCKS * 4096u, stLit>>>(src, srcSize, blocks, nBlocks, lits, hufTabs, litJobs); }
-    { uint32_t grid = (nBlocks + D1_WARPS(1) - 1) / D1_WARPS(1); if (grid > cap) grid = cap;
-      zstd_dec_entropy_kernel<1><<<grid, D1_WARPS(1) * 32, 0, st>>>(src, srcSize, blocks, nBlocks, lits, hufTabs, litJobs, seqTabs, seqJobs);
-      zstd_dec_seq_streams_kernel<<<(nBlocks + 127u) / 128u, 128, 0, st>>>(src, srcSize, blocks, nBlocks, seqs, seqTabs, seqJobs); }
+      cudaFuncSetAttribute(zstd_dec_lit_streams_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+      zstd_dec_lit_streams_kernel<<<(nBlocks + B2Z_LIT_BLOCKS - 1u) / B2Z_LIT_BLOCKS, B2Z_LIT_BLOCKS * 4u, B2Z_LIT_BLOCKS * 4096u, stLit>>>(src, srcSize, blocks, nBlocks, lits, nullptr, litJobs); }
+    { const uint32_t threads = D1_WARPS(1) * 32;
+      zstd_dec_entropy_kernel<1><<<(nBlocks + threads - 1) / threads, threads, 0, st>>>(src, srcSize, blocks, nBlocks, lits, nullptr, litJobs, nullptr, seqJobs);
+      cudaFuncSetAttribute(zstd_dec_seq_streams_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+      zstd_dec_seq_streams_kernel<<<(nBlocks + B2Z_SEQ_BLOCKS - 1u) / B2Z_SEQ_BLOCKS, 32, 0, st>>>(src, srcSize, blocks, nBlocks, seqs, nullptr, seqJobs); }   // one warp: B2Z_SEQ_BLOCKS chains
     if (stLit != st) { cudaEventRecord(evJoin, stLit); cudaStreamWaitEvent(st, evJoin, 0); }
 }
-size_t zstd_dec_entropy_scratch_bytes(uint32_t nBlocks) { return (size_t)nBlocks * (4096u + 1280u * sizeof(SeqEnt) + sizeof(LitJob) + sizeof(SeqJob)) + 256u; }
+size_t zstd_dec_entropy_scratch_bytes(uint32_t nBlocks) { return (size_t)nBlocks * (sizeof(LitJob) + sizeof(SeqJob)) + 256u; }
 void launch_zstd_dec_layout(DecFrame* frames, uint32_t nFrames, DecBlock* blocks, uint64_t dstCap, DecCounts* counts, uint64_t* total, uint32_t jumpMode, cudaStream_t st) {
     if (nFrames) zstd_dec_frame_sizes_kernel<<<(nFrames + 127) / 128, 128, 0, st>>>(frames, nFrames, blocks, counts, jumpMode);
     zstd_dec_frame_offsets_kernel<<<1, 32, 0, st>>>(frames, nFrames, dstCap, counts, total);
