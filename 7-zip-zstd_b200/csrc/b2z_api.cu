@@ -6,9 +6,6 @@
 // :1853, ZSTDMT_createCompressionJob :1403, ZSTDMT_flushProduced :1488): frames are the jobs,
 // warps are the workers, the assemble kernels are the ordered flush.
 #include <vector>
-#include <thread>
-#include <mutex>
-#include <condition_variable>
 #include "b2z_ctx.h"
 #include "b2z_lzma2.h"
 #include "b2z_lzma_model.h"
@@ -277,6 +274,7 @@ static int enc_batch(b200z_ctx* ctx, const uint8_t* d_src, uint64_t n, uint8_t* 
     // blocks are numbered per frame with a fixed stride (frames are multiples of 128 KiB)
     cudaStream_t st = ctx->stream;
     uint32_t* const errFlag = (uint32_t*)ctx->scalars.p + 16;
+    auto addMs = [&](int s, int from, int to) { float ms = 0; cudaEventElapsedTime(&ms, ctx->ev[from], ctx->ev[to]); ctx->stat[s] += ms; };
     CU(cudaMemsetAsync(ctx->scalars.p, 0, 128, st));
     CU(cudaEventRecord(ctx->ev[0], st));
     if (price_parse(g, codec)) {
@@ -290,13 +288,6 @@ static int enc_batch(b200z_ctx* ctx, const uint8_t* d_src, uint64_t n, uint8_t* 
                                       (uint8_t*)ctx->lits.p, (uint32_t*)ctx->nlit.p, st));
         CU(cudaEventRecord(ctx->ev[1], st));
         ctx->stat[B200Z_S_KERNEL_LAUNCHES] += 2;
-        if (stageMOnly) {
-            CU(cudaStreamSynchronize(st));
-            float ms = 0;
-            cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[4]); ctx->stat[B200Z_S_ENC_MATCH_MS] += ms;
-            cudaEventElapsedTime(&ms, ctx->ev[4], ctx->ev[1]); ctx->stat[B200Z_S_ENC_PARSE_MS] += ms;
-            return 0;
-        }
     } else {
         EncGeom gF = g;                                                 // stage F's unit: the frame, or the region of a long frame
         if (long_mode(g, codec)) gF.frameLog = g.regionLog;
@@ -311,7 +302,12 @@ static int enc_batch(b200z_ctx* ctx, const uint8_t* d_src, uint64_t n, uint8_t* 
         CU(cudaEventRecord(ctx->ev[1], st));
         ctx->stat[B200Z_S_KERNEL_LAUNCHES] += 2;
     }
-    if (!stageMOnly && codec == 1) {
+    if (stageMOnly) {
+        CU(cudaStreamSynchronize(st));
+        addMs(B200Z_S_ENC_MATCH_MS, 0, 4); addMs(B200Z_S_ENC_PARSE_MS, 4, 1);
+        return 0;
+    }
+    if (codec == 1) {
         // LZMA2: stage R (range coding, one thread per frame) + assembly of the frame slots into one chunk stream
         const uint32_t LITN = b2z_lz2_litn(b2z_lz2_props(g.flags));
         uint16_t* spill = nullptr;
@@ -332,44 +328,114 @@ static int enc_batch(b200z_ctx* ctx, const uint8_t* d_src, uint64_t n, uint8_t* 
         CU(cudaEventRecord(ctx->ev[2], st));
         launch_lzma2_enc_assemble((const uint8_t*)ctx->slots.p, (const uint32_t*)ctx->slotSize.p, (uint32_t)nChains, (uint32_t)lzma2_enc_slot_stride(g),
                                   (uint64_t*)ctx->frameOff.p, d_dst, (uint64_t*)ctx->scalars.p, st);
-        CU(cudaGetLastError());
-        CU(cudaEventRecord(ctx->ev[3], st));
-        ctx->stat[B200Z_S_KERNEL_LAUNCHES] += 3;
-        uint64_t hs[9] = {0};
-        { const int frc = b2z_fetch_small(ctx, hs, ctx->scalars.p, 72, st); if (frc) return frc; }
-        if ((uint32_t)hs[8]) return fail(ctx, B200Z_E_CUDA, "upload stalled: an input chunk never arrived%s");
-        if ((uint32_t)hs[2]) return fail(ctx, B200Z_E_CUDA, "LZMA2: frame slot overflow%s");
-        *produced = hs[0];
-        float ms = 0;
-        cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[4]); ctx->stat[B200Z_S_ENC_MATCH_MS] += ms;
-        cudaEventElapsedTime(&ms, ctx->ev[4], ctx->ev[1]); ctx->stat[B200Z_S_ENC_PARSE_MS] += ms;
-        cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]); ctx->stat[B200Z_S_ENC_ENTROPY_MS] += ms;
-        cudaEventElapsedTime(&ms, ctx->ev[2], ctx->ev[3]); ctx->stat[B200Z_S_ENC_ASSEMBLE_MS] += ms;
-    } else if (!stageMOnly) {
+    } else {
         launch_zstd_enc_entropy(d_src, n, g, (const uint64_t*)ctx->seqs.p, (const uint32_t*)ctx->nseq.p, (const uint8_t*)ctx->lits.p,
                                 (const uint32_t*)ctx->nlit.p, (uint8_t*)ctx->slots.p, (uint32_t*)ctx->slotSize.p, nBlocks, ctx->smCount, st);
         CU(cudaGetLastError());
         CU(cudaEventRecord(ctx->ev[2], st));
         launch_zstd_enc_assemble(d_src, n, g, (const uint8_t*)ctx->slots.p, (const uint32_t*)ctx->slotSize.p, nBlocks, (uint64_t*)ctx->blockOff.p,
                                  d_dst, (uint64_t*)ctx->scalars.p, (uint64_t*)ctx->frameOff.p, (uint32_t*)ctx->cks.p, st);
-        CU(cudaGetLastError());
-        CU(cudaEventRecord(ctx->ev[3], st));
-        ctx->stat[B200Z_S_KERNEL_LAUNCHES] += 3;
-        uint64_t hs[9] = {0};
-        { const int frc = b2z_fetch_small(ctx, hs, ctx->scalars.p, 72, st); if (frc) return frc; }
-        if ((uint32_t)hs[8]) return fail(ctx, B200Z_E_CUDA, "upload stalled: an input chunk never arrived%s");
-        *produced = hs[0];
-        float ms = 0;
-        cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[4]); ctx->stat[B200Z_S_ENC_MATCH_MS] += ms;
-        cudaEventElapsedTime(&ms, ctx->ev[4], ctx->ev[1]); ctx->stat[B200Z_S_ENC_PARSE_MS] += ms;
-        cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]); ctx->stat[B200Z_S_ENC_ENTROPY_MS] += ms;
-        cudaEventElapsedTime(&ms, ctx->ev[2], ctx->ev[3]); ctx->stat[B200Z_S_ENC_ASSEMBLE_MS] += ms;
-    } else {
-        CU(cudaStreamSynchronize(st));
-        float ms = 0;
-        cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[4]); ctx->stat[B200Z_S_ENC_MATCH_MS] += ms;
-        cudaEventElapsedTime(&ms, ctx->ev[4], ctx->ev[1]); ctx->stat[B200Z_S_ENC_PARSE_MS] += ms;
     }
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(ctx->ev[3], st));
+    ctx->stat[B200Z_S_KERNEL_LAUNCHES] += 3;
+    uint64_t hs[9] = {0};
+    { const int frc = b2z_fetch_small(ctx, hs, ctx->scalars.p, 72, st); if (frc) return frc; }
+    if ((uint32_t)hs[8]) return fail(ctx, B200Z_E_CUDA, "upload stalled: an input chunk never arrived%s");
+    if (codec == 1 && (uint32_t)hs[2]) return fail(ctx, B200Z_E_CUDA, "LZMA2: frame slot overflow%s");
+    *produced = hs[0];
+    addMs(B200Z_S_ENC_MATCH_MS, 0, 4); addMs(B200Z_S_ENC_PARSE_MS, 4, 1); addMs(B200Z_S_ENC_ENTROPY_MS, 1, 2); addMs(B200Z_S_ENC_ASSEMBLE_MS, 2, 3);
+    return 0;
+}
+
+// bytes per batch of a call that codes 2^log at a time: at most 1 GiB for the price-based parses (stage C keeps 16 bytes per input
+// byte), at least one frame
+static uint64_t batch_bytes(const b200z_ctx* ctx, uint32_t log, int codec) {
+    const uint64_t F = 1ull << ctx->geom.frameLog;
+    uint64_t batch = 1ull << log;
+    if ((ctx->geom.flags & (codec == 1 ? B2Z_FLAG_LZ2_OPT : B2Z_FLAG_ZSTD_OPT)) && batch > (1ull << 30)) batch = 1ull << 30;
+    return batch < F ? F : batch;
+}
+
+// device-pointer compress of srcSize > 0 bytes: batches of whole frames, one after the other.  LZMA2 (codec 1): the chunks of the next
+// batch follow directly, over the end marker of the one before.
+static int enc_device_batches(b200z_ctx* ctx, const uint8_t* d_src, uint64_t srcSize, uint8_t* d_dst, int codec, size_t* dstSize) {
+    const uint64_t batch = batch_bytes(ctx, ctx->batchLog, codec);
+    uint64_t done = 0, outPos = 0;
+    while (done < srcSize) {
+        const uint64_t n = (srcSize - done) < batch ? (srcSize - done) : batch;
+        uint64_t produced = 0;
+        const int rc = enc_batch(ctx, d_src + done, n, d_dst + outPos, &produced, false, nullptr, 0, codec);
+        if (rc) return rc;
+        done += n; outPos += produced;
+        if (codec == 1 && done < srcSize) outPos -= 1;
+    }
+    *dstSize = (size_t)outPos;
+    return 0;
+}
+
+// Host-pointer upload of n > 0 bytes to d_dst in <= 16 chunks of >= 1 MiB on stream2, each followed by its flag in ctx->ready: the
+// kernels start at once and stage F's CTAs wait for their chunk, so the H2D time hides under the match kernel.  *shift: log2 of the
+// chunk size, which enc_batch takes.
+static int upload_chunked(b200z_ctx* ctx, uint8_t* d_dst, const uint8_t* src, uint64_t n, uint32_t* shift) {
+    if (ctx->ready.reserve(256)) return fail(ctx, B200Z_E_MEMORY, "device staging allocation failed%s");
+    if (!ctx->hostOne) { if (cudaHostAlloc((void**)&ctx->hostOne, 64, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); return fail(ctx, B200Z_E_MEMORY, "pinned allocation failed%s"); } *ctx->hostOne = 1u; }
+    uint32_t s = 20; while (((n - 1) >> s) >= 16) s++;
+    const uint32_t nChunks = (uint32_t)(((n - 1) >> s) + 1);
+    CU(cudaMemsetAsync(ctx->ready.p, 0, 256, ctx->stream));
+    CU(cudaEventRecord(ctx->pe[0], ctx->stream));
+    CU(cudaStreamWaitEvent(ctx->stream2, ctx->pe[0], 0));
+    for (uint32_t c = 0; c < nChunks; c++) {
+        const size_t off = (size_t)c << s, len = (n - off) < ((size_t)1 << s) ? (n - off) : ((size_t)1 << s);
+        CU(cudaMemcpyAsync(d_dst + off, src + off, len, cudaMemcpyHostToDevice, ctx->stream2));
+        CU(cudaMemcpyAsync((uint32_t*)ctx->ready.p + c, ctx->hostOne, 4, cudaMemcpyHostToDevice, ctx->stream2));
+    }
+    *shift = s;
+    return 0;
+}
+
+static size_t enc_bound(b200z_ctx* ctx, uint64_t n, int codec) { return codec == 1 ? b200z_lzma2_compress_bound(ctx, n) : b200z_zstd_compress_bound(ctx, n); }
+
+// Host-pointer compress on one device, batch after batch: chunked upload, kernels, download.  srcSize == 0 (zstd only): the empty frame.
+static int enc_host_serial(b200z_ctx* ctx, const uint8_t* src, uint64_t srcSize, uint8_t* dst, uint64_t batch, int codec, size_t* dstSize) {
+    const uint64_t maxIn = srcSize < batch ? srcSize : batch;
+    const size_t bound = enc_bound(ctx, maxIn, codec);
+    if (ctx->dIn.reserve(maxIn + 64) || ctx->dOut.reserve(bound)) return fail(ctx, B200Z_E_MEMORY, "device staging allocation failed%s");
+    uint8_t* const dIn = (uint8_t*)ctx->dIn.p; uint8_t* const dOut = (uint8_t*)ctx->dOut.p;
+    uint64_t done = 0, outPos = 0;
+    do {
+        const uint64_t n = (srcSize - done) < batch ? (srcSize - done) : batch;
+        uint64_t produced = 0;
+        if (n == 0) { size_t o = 0; const int rc = b200z_zstd_compress_device(ctx, dIn, 0, dOut, bound, &o); if (rc) return rc; produced = o; }
+        else {
+            uint32_t shift = 0;
+            int rc = upload_chunked(ctx, dIn, src + done, n, &shift);
+            if (!rc) rc = enc_batch(ctx, dIn, n, dOut, &produced, false, (const uint32_t*)ctx->ready.p, shift, codec);
+            if (rc) { cudaStreamSynchronize(ctx->stream2); return rc; }
+        }
+        if (codec == 1 && done + n < srcSize) produced -= 1;            // the next batch's chunks follow directly: no end marker in between
+        CU(cudaMemcpyAsync(dst + outPos, dOut, produced, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        ctx->stat[B200Z_S_H2D_BYTES] += (double)n; ctx->stat[B200Z_S_D2H_BYTES] += (double)produced;
+        done += n; outPos += produced;
+    } while (done < srcSize);
+    *dstSize = (size_t)outPos;
+    return 0;
+}
+
+// Host-pointer compress through the batch pipeline (b2z_host_pipeline): batch i of `batch` bytes goes to device i mod N.
+static int enc_host_pipelined(b200z_ctx* ctx, const uint8_t* src, uint64_t srcSize, uint8_t* dst, uint64_t batch, int codec, size_t* dstSize) {
+    std::vector<HostBatch> batches;
+    for (uint64_t off = 0; off < srcSize; off += batch) batches.push_back({ (size_t)off, (size_t)((srcSize - off) < batch ? (srcSize - off) : batch), 0, false });
+    const size_t outStride = (enc_bound(ctx, batch, codec) + 255) & ~(size_t)255;
+    uint64_t total = 0;
+    const int rc = b2z_host_pipeline(ctx, src, dst, batches, batch + 64, outStride, [&](b200z_ctx* c, size_t i, const uint8_t* dIn, uint8_t* dOut, uint64_t* out) {
+        const int brc = enc_batch(c, dIn, batches[i].srcLen, dOut, out, false, nullptr, 0, codec);
+        if (!brc && codec == 1 && i + 1 < batches.size()) *out -= 1;  // the next batch's chunks follow directly: no end marker in between
+        return brc;
+    }, &total);
+    if (rc) return rc;
+    *dstSize = (size_t)total;
     return 0;
 }
 
@@ -395,95 +461,18 @@ int b200z_zstd_compress_device(b200z_ctx* ctx, const void* d_src, size_t srcSize
         CU(cudaStreamSynchronize(ctx->stream));
         *dstSize = o; return 0;
     }
-    // batches are whole frames
-    const uint64_t F = 1ull << ctx->geom.frameLog;
-    uint64_t batch = 1ull << ctx->batchLog;
-    if ((ctx->geom.flags & B2Z_FLAG_ZSTD_OPT) && batch > (1ull << 30)) batch = 1ull << 30;   // stage C keeps 16 bytes per input byte
-    if (batch < F) batch = F;
-    uint64_t done = 0, outPos = 0;
-    while (done < srcSize) {
-        const uint64_t n = (srcSize - done) < batch ? (srcSize - done) : batch;
-        uint64_t produced = 0;
-        int rc = enc_batch(ctx, (const uint8_t*)d_src + done, n, (uint8_t*)d_dst + outPos, &produced, false);
-        if (rc) return rc;
-        done += n; outPos += produced;
-    }
-    *dstSize = (size_t)outPos;
-    return 0;
+    return enc_device_batches(ctx, (const uint8_t*)d_src, srcSize, (uint8_t*)d_dst, 0, dstSize);
 }
 
-// ---- a host-pointer compress shared by the devices of a context
-struct EncJob {
-    const uint8_t* src = nullptr; size_t srcSize = 0; uint8_t* dst = nullptr; uint64_t batch = 0, nItems = 0;
-    int codec = 0;                                               // 0 zstd frames; 1 LZMA2 chunk stream (every batch but the last drops its end marker)
-    std::mutex m; std::condition_variable cv;
-    std::vector<uint64_t> size; std::vector<char> known;         // compressed bytes of every batch, once known
-    int rc = 0; b200z_ctx* errCtx = nullptr;                     // first error
-    void fail_with(int code, b200z_ctx* c) { std::lock_guard<std::mutex> g(m); if (!rc) { rc = code; errCtx = c; } cv.notify_all(); }
-    void publish(uint64_t i, uint64_t n) { std::lock_guard<std::mutex> g(m); size[i] = n; known[i] = 1; cv.notify_all(); }
-    // output offset of batch i: blocks until the sizes of batches 0 .. i-1 are known; false when another device failed
-    bool offset_of(uint64_t i, uint64_t* off) {
-        std::unique_lock<std::mutex> g(m);
-        uint64_t sum = 0;
-        for (uint64_t k = 0; k < i; k++) { cv.wait(g, [&] { return rc != 0 || known[k]; }); if (rc) return false; sum += size[k]; }
-        *off = sum; return true;
-    }
-};
-
-// one device's share: batches first, first + stride, ... through  H2D (stream2) | kernels (stream) | D2H (stream3), double-buffered
-static void enc_worker(b200z_ctx* ctx, EncJob* job, uint64_t first, uint64_t stride) {
-    auto run = [&]() -> int {
-        CU(cudaSetDevice(ctx->device));
-        const uint64_t batch = job->batch;
-        const size_t batchBound = ((job->codec == 1 ? b200z_lzma2_compress_bound(ctx, batch) : b200z_zstd_compress_bound(ctx, batch)) + 255) & ~(size_t)255;
-        if (ctx->dIn.reserve(2 * (batch + 64)) || ctx->dOut.reserve(2 * batchBound)) return fail(ctx, B200Z_E_MEMORY, "device staging allocation failed%s");
-        uint8_t* dIn[2] = { (uint8_t*)ctx->dIn.p, (uint8_t*)ctx->dIn.p + batch + 64 };
-        uint8_t* dOut[2] = { (uint8_t*)ctx->dOut.p, (uint8_t*)ctx->dOut.p + batchBound };
-        auto bsize = [&](uint64_t i) { return (size_t)((job->srcSize - i * batch) < batch ? (job->srcSize - i * batch) : batch); };
-        // pe[0..1]: input of buffer b uploaded; pe[2..3]: output of buffer b downloaded
-        CU(cudaMemcpyAsync(dIn[0], job->src + first * batch, bsize(first), cudaMemcpyHostToDevice, ctx->stream2));
-        CU(cudaEventRecord(ctx->pe[0], ctx->stream2));
-        uint64_t k = 0;
-        for (uint64_t i = first; i < job->nItems; i += stride, k++) {
-            const int b = (int)(k & 1);
-            if (i + stride < job->nItems) {                          // upload the next batch while this one is compressed
-                // its buffer was last read by the kernels of the batch before this one, which have been synchronised already
-                CU(cudaMemcpyAsync(dIn[b ^ 1], job->src + (i + stride) * batch, bsize(i + stride), cudaMemcpyHostToDevice, ctx->stream2));
-                CU(cudaEventRecord(ctx->pe[b ^ 1], ctx->stream2));
-            }
-            CU(cudaStreamWaitEvent(ctx->stream, ctx->pe[b], 0));                 // input there
-            if (k >= 2) CU(cudaStreamWaitEvent(ctx->stream, ctx->pe[2 + b], 0)); // output buffer drained
-            uint64_t produced = 0;
-            int rc = enc_batch(ctx, dIn[b], bsize(i), dOut[b], &produced, false, nullptr, 0, job->codec);   // synchronises ctx->stream
-            if (rc) return rc;
-            if (job->codec == 1 && i + 1 < job->nItems) produced -= 1;            // the next batch's chunks follow directly: no end marker in between
-            job->publish(i, produced);
-            uint64_t off = 0;
-            if (!job->offset_of(i, &off)) return 0;                              // another device failed: its error is the job's
-            CU(cudaMemcpyAsync(job->dst + off, dOut[b], produced, cudaMemcpyDeviceToHost, ctx->stream3));
-            CU(cudaEventRecord(ctx->pe[2 + b], ctx->stream3));
-            ctx->stat[B200Z_S_H2D_BYTES] += (double)bsize(i); ctx->stat[B200Z_S_D2H_BYTES] += (double)produced;
-        }
-        CU(cudaStreamSynchronize(ctx->stream3));
-        return 0;
-    };
-    const int rc = run();
-    if (rc) job->fail_with(rc, ctx);
-}
-
-// Host-pointer compress: the stream is cut into batches of whole frames that flow through a three-stage
-// pipeline -- H2D copy of batch i+1 (stream2) | kernels of batch i (stream) | D2H copy of batch i-1 (stream3) --
-// with double-buffered device staging, so PCIe time hides under kernel time when the host buffers are pinned.
-// (The ordered output mirrors ZSTDMT_flushProduced, zstdmt_compress.c:1488.)
+// Host-pointer compress: one batch on one device (and the empty input) takes the chunked upload; several batches and / or several
+// devices take the pipeline, H2D copy of batch i+1 | kernels of batch i | D2H copy of batch i-1 on every device.
 int b200z_zstd_compress_host(b200z_ctx* ctx, const void* src, size_t srcSize, void* dst, size_t dstCap, size_t* dstSize) {
     if (!ctx || !dstSize || (!src && srcSize) || !dst) return B200Z_E_PARAM;
-    const size_t bound = b200z_zstd_compress_bound(ctx, srcSize);
-    if (dstCap < bound) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_zstd_compress_bound%s");
+    if (dstCap < b200z_zstd_compress_bound(ctx, srcSize)) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_zstd_compress_bound%s");
     CU(cudaSetDevice(ctx->device));
     const uint64_t F = 1ull << ctx->geom.frameLog;
     const uint64_t nDev = 1 + ctx->peers.size();
-    uint64_t batch = 1ull << ctx->hostBatchLog;
-    if ((ctx->geom.flags & B2Z_FLAG_ZSTD_OPT) && batch > (1ull << 30)) batch = 1ull << 30;
+    uint64_t batch = batch_bytes(ctx, ctx->hostBatchLog, 0);
     if (nDev > 1) {                                              // about four batches per device, none smaller than one frame per SM
         const uint64_t unit = long_mode(ctx->geom, 0) ? 1ull << ctx->geom.regionLog : F;        // what one CTA of stage F takes
         uint64_t per = (srcSize + 4 * nDev - 1) / (4 * nDev), floorB = (uint64_t)ctx->smCount * unit;
@@ -491,54 +480,12 @@ int b200z_zstd_compress_host(b200z_ctx* ctx, const void* src, size_t srcSize, vo
         per = (per + F - 1) / F * F;
         if (per < batch) batch = per;
     }
-    if (batch < F) batch = F;
     {   // whole rounds of stage F's grid (one CTA per SM, one region each): a batch of 1024 regions would end with a partial round (1024 = 7 x 132 + 100 on an H100)
         const uint64_t unit = long_mode(ctx->geom, 0) ? 1ull << ctx->geom.regionLog : F, round = (uint64_t)ctx->smCount * unit;
         if (!(ctx->geom.flags & B2Z_FLAG_ZSTD_OPT) && batch > round && srcSize > batch) { const uint64_t b = batch / round * round; if (b % F == 0) batch = b; }
     }
-    if (nDev == 1 && srcSize <= batch) {
-        // one batch: the upload is cut into chunks on stream2, each followed by a flag write; stage M starts at once and
-        // its frame-warps wait for their chunk, so the H2D time hides under the match kernel
-        if (ctx->dIn.reserve(srcSize + 64) || ctx->dOut.reserve(bound) || ctx->ready.reserve(256)) return fail(ctx, B200Z_E_MEMORY, "device staging allocation failed%s");
-        if (!ctx->hostOne) { if (cudaHostAlloc((void**)&ctx->hostOne, 64, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); return fail(ctx, B200Z_E_MEMORY, "pinned allocation failed%s"); } *ctx->hostOne = 1u; }
-        size_t out = 0;
-        if (srcSize == 0) { int rc = b200z_zstd_compress_device(ctx, ctx->dIn.p, 0, ctx->dOut.p, bound, &out); if (rc) return rc; }
-        else {
-            uint32_t shift = 20; while (((srcSize - 1) >> shift) >= 16) shift++;          // <= 16 chunks of >= 1 MiB
-            const uint32_t nChunks = (uint32_t)(((srcSize - 1) >> shift) + 1);
-            CU(cudaMemsetAsync(ctx->ready.p, 0, 256, ctx->stream));
-            CU(cudaEventRecord(ctx->pe[0], ctx->stream));
-            CU(cudaStreamWaitEvent(ctx->stream2, ctx->pe[0], 0));
-            for (uint32_t c = 0; c < nChunks; c++) {
-                const size_t off = (size_t)c << shift, len = (srcSize - off) < ((size_t)1 << shift) ? (srcSize - off) : ((size_t)1 << shift);
-                CU(cudaMemcpyAsync((uint8_t*)ctx->dIn.p + off, (const uint8_t*)src + off, len, cudaMemcpyHostToDevice, ctx->stream2));
-                CU(cudaMemcpyAsync((uint32_t*)ctx->ready.p + c, ctx->hostOne, 4, cudaMemcpyHostToDevice, ctx->stream2));
-            }
-            uint64_t produced = 0;
-            int rc = enc_batch(ctx, (const uint8_t*)ctx->dIn.p, srcSize, (uint8_t*)ctx->dOut.p, &produced, false, (const uint32_t*)ctx->ready.p, shift, 0);
-            if (rc) { cudaStreamSynchronize(ctx->stream2); return rc; }
-            out = (size_t)produced;
-        }
-        ctx->stat[B200Z_S_H2D_BYTES] += (double)srcSize;
-        CU(cudaMemcpyAsync(dst, ctx->dOut.p, out, cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        ctx->stat[B200Z_S_D2H_BYTES] += (double)out;
-        *dstSize = out;
-        return 0;
-    }
-    // several batches and / or several devices: batch i goes to device i mod N; every device runs the three-stage pipeline over its
-    // batches, and a batch's download starts once the sizes of all earlier batches are known (they are dealt in order, so that is soon)
-    EncJob job; job.src = (const uint8_t*)src; job.srcSize = srcSize; job.dst = (uint8_t*)dst; job.batch = batch;
-    job.nItems = (srcSize + batch - 1) / batch; job.size.assign(job.nItems, 0); job.known.assign(job.nItems, 0);
-    const uint64_t nWorkers = nDev < job.nItems ? nDev : job.nItems;
-    std::vector<std::thread> threads;
-    for (uint64_t d = 1; d < nWorkers; d++) threads.emplace_back(enc_worker, ctx->peers[d - 1], &job, d, nWorkers);
-    enc_worker(ctx, &job, 0, nWorkers);
-    for (std::thread& t : threads) t.join();
-    if (job.rc) { if (job.errCtx && job.errCtx != ctx) snprintf(ctx->err, sizeof(ctx->err), "device %d: %.200s", job.errCtx->device, job.errCtx->err); return job.rc; }
-    size_t total = 0; for (uint64_t v : job.size) total += (size_t)v;
-    *dstSize = total;
-    return 0;
+    if (srcSize == 0 || (nDev == 1 && srcSize <= batch)) return enc_host_serial(ctx, (const uint8_t*)src, srcSize, (uint8_t*)dst, batch, 0, dstSize);
+    return enc_host_pipelined(ctx, (const uint8_t*)src, srcSize, (uint8_t*)dst, batch, 0, dstSize);
 }
 
 int b200z_zstd_enc_stage_m(b200z_ctx* ctx, const void* d_src, size_t srcSize, uint64_t* seqs, uint32_t* nseq, uint8_t* lits, uint32_t* nlit) {
@@ -687,22 +634,12 @@ int b200z_lzma2_compress_device(b200z_ctx* ctx, const void* d_src, size_t srcSiz
     if (dstCap < b200z_lzma2_compress_bound(ctx, srcSize)) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_lzma2_compress_bound%s");
     if (dictProp) *dictProp = (ctx->geom.frameLog - 12u) * 2u;           // dictionary = frame size (Lzma2Enc_WriteProperties, Lzma2Enc.c:671)
     CU(cudaSetDevice(ctx->device));
-    const uint64_t F = 1ull << ctx->geom.frameLog;
-    uint64_t batch = 1ull << ctx->batchLog;
-    if ((ctx->geom.flags & B2Z_FLAG_LZ2_OPT) && batch > (1ull << 30)) batch = 1ull << 30;    // stage C keeps 16 bytes per input byte
-    if (batch < F) batch = F;
-    uint64_t done = 0, outPos = 0;
-    while (done < srcSize) {
-        const uint64_t n = (srcSize - done) < batch ? (srcSize - done) : batch;
-        uint64_t produced = 0;
-        int rc = enc_batch(ctx, (const uint8_t*)d_src + done, n, (uint8_t*)d_dst + outPos, &produced, false, nullptr, 0, 1);
-        if (rc) return rc;
-        done += n; outPos += produced - 1;                               // the next batch overwrites this batch's end marker
+    if (srcSize == 0) {                                                  // the end marker alone
+        CU(cudaMemsetAsync(d_dst, 0, 1, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        *dstSize = 1; return 0;
     }
-    if (!srcSize) CU(cudaMemsetAsync(d_dst, 0, 1, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    *dstSize = (size_t)outPos + 1;
-    return 0;
+    return enc_device_batches(ctx, (const uint8_t*)d_src, srcSize, (uint8_t*)d_dst, 1, dstSize);
 }
 
 // Test tap of the price-based parse: stage C's candidate words and stage P's per-block sequences of a device buffer (one batch)
@@ -722,19 +659,17 @@ int b200z_lzma2_enc_stage_cp(b200z_ctx* ctx, const void* d_src, size_t srcSize, 
     return 0;
 }
 
-// Host-pointer form; one batch: chunked upload overlapped with stage M (as the zstd path), kernels, download.
+// Host-pointer form: batches of whole dictionary-reset blocks, dealt over the devices by the pipeline (the role of MtCoder_Code,
+// MtCoder.c:445, one level up), or on one device one after the other, each with the chunked upload.
 int b200z_lzma2_compress_host(b200z_ctx* ctx, const void* src, size_t srcSize, void* dst, size_t dstCap, size_t* dstSize, uint32_t* dictProp) {
     if (!ctx || !dstSize || (!src && srcSize) || !dst) return B200Z_E_PARAM;
     { const int prc = lz2_check_props(ctx); if (prc) return prc; }
-    const size_t bound = b200z_lzma2_compress_bound(ctx, srcSize);
-    if (dstCap < bound) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_lzma2_compress_bound%s");
+    if (dstCap < b200z_lzma2_compress_bound(ctx, srcSize)) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_lzma2_compress_bound%s");
     if (dictProp) *dictProp = (ctx->geom.frameLog - 12u) * 2u;
     if (!srcSize) { *(uint8_t*)dst = 0; *dstSize = 1; return 0; }
     CU(cudaSetDevice(ctx->device));
     const uint64_t F = 1ull << ctx->geom.frameLog;
-    uint64_t batch = 1ull << ctx->hostBatchLog;
-    if ((ctx->geom.flags & B2Z_FLAG_LZ2_OPT) && batch > (1ull << 30)) batch = 1ull << 30;
-    if (batch < F) batch = F;
+    uint64_t batch = batch_bytes(ctx, ctx->hostBatchLog, 1);
     const uint64_t nDev = 1 + ctx->peers.size();
     if (nDev > 1) {                                              // about four batches per device, none smaller than a frame per SM (or 16 frames for large frames)
         uint64_t per = (srcSize + 4 * nDev - 1) / (4 * nDev), floorB = (F >= (1ull << 23) ? 16ull : (uint64_t)ctx->smCount) * F;
@@ -742,47 +677,8 @@ int b200z_lzma2_compress_host(b200z_ctx* ctx, const void* src, size_t srcSize, v
         per = (per + F - 1) / F * F;
         if (per < batch) batch = per;
     }
-    if (nDev > 1 && srcSize > batch) {
-        // batches of whole dictionary-reset blocks dealt over the devices (the role of MtCoder_Code, MtCoder.c:445, one level up)
-        EncJob job; job.src = (const uint8_t*)src; job.srcSize = srcSize; job.dst = (uint8_t*)dst; job.batch = batch; job.codec = 1;
-        job.nItems = (srcSize + batch - 1) / batch; job.size.assign(job.nItems, 0); job.known.assign(job.nItems, 0);
-        const uint64_t nWorkers = nDev < job.nItems ? nDev : job.nItems;
-        std::vector<std::thread> threads;
-        for (uint64_t d = 1; d < nWorkers; d++) threads.emplace_back(enc_worker, ctx->peers[d - 1], &job, d, nWorkers);
-        enc_worker(ctx, &job, 0, nWorkers);
-        for (std::thread& t : threads) t.join();
-        if (job.rc) { if (job.errCtx && job.errCtx != ctx) snprintf(ctx->err, sizeof(ctx->err), "device %d: %.200s", job.errCtx->device, job.errCtx->err); return job.rc; }
-        size_t total = 0; for (uint64_t v : job.size) total += (size_t)v;
-        *dstSize = total;
-        return 0;
-    }
-    const uint64_t maxIn = srcSize < batch ? srcSize : batch;
-    if (ctx->dIn.reserve(maxIn + 64) || ctx->dOut.reserve(b200z_lzma2_compress_bound(ctx, maxIn)) || ctx->ready.reserve(256))
-        return fail(ctx, B200Z_E_MEMORY, "device staging allocation failed%s");
-    if (!ctx->hostOne) { if (cudaHostAlloc((void**)&ctx->hostOne, 64, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); return fail(ctx, B200Z_E_MEMORY, "pinned allocation failed%s"); } *ctx->hostOne = 1u; }
-    uint64_t done = 0, outPos = 0;
-    while (done < srcSize) {
-        const uint64_t n = (srcSize - done) < batch ? (srcSize - done) : batch;
-        uint32_t shift = 20; while (((n - 1) >> shift) >= 16) shift++;
-        const uint32_t nChunks = (uint32_t)(((n - 1) >> shift) + 1);
-        CU(cudaMemsetAsync(ctx->ready.p, 0, 256, ctx->stream));
-        CU(cudaEventRecord(ctx->pe[0], ctx->stream));
-        CU(cudaStreamWaitEvent(ctx->stream2, ctx->pe[0], 0));
-        for (uint32_t c = 0; c < nChunks; c++) {
-            const size_t off = (size_t)c << shift, len = (n - off) < ((size_t)1 << shift) ? (n - off) : ((size_t)1 << shift);
-            CU(cudaMemcpyAsync((uint8_t*)ctx->dIn.p + off, (const uint8_t*)src + done + off, len, cudaMemcpyHostToDevice, ctx->stream2));
-            CU(cudaMemcpyAsync((uint32_t*)ctx->ready.p + c, ctx->hostOne, 4, cudaMemcpyHostToDevice, ctx->stream2));
-        }
-        uint64_t produced = 0;
-        int rc = enc_batch(ctx, (const uint8_t*)ctx->dIn.p, n, (uint8_t*)ctx->dOut.p, &produced, false, (const uint32_t*)ctx->ready.p, shift, 1);
-        if (rc) { cudaStreamSynchronize(ctx->stream2); return rc; }
-        CU(cudaMemcpyAsync((uint8_t*)dst + outPos, ctx->dOut.p, produced, cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        ctx->stat[B200Z_S_H2D_BYTES] += (double)n; ctx->stat[B200Z_S_D2H_BYTES] += (double)produced;
-        done += n; outPos += produced - 1;
-    }
-    *dstSize = (size_t)outPos + 1;
-    return 0;
+    return nDev > 1 && srcSize > batch ? enc_host_pipelined(ctx, (const uint8_t*)src, srcSize, (uint8_t*)dst, batch, 1, dstSize)
+                                       : enc_host_serial(ctx, (const uint8_t*)src, srcSize, (uint8_t*)dst, batch, 1, dstSize);
 }
 
 // ---------------------------------------------------------------- device memory helpers

@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <new>
 #include <vector>
 #include "../../include/b200z.h"
@@ -61,6 +62,17 @@ static inline int fail(b200z_ctx* c, int code, const char* fmt, const char* deta
 // (A cudaMemcpyAsync of a few bytes queues behind whatever the device-to-host engine is doing -- in the host-pointer pipelines the
 // gigabyte download of the previous batch: measured, the kernels of batch k+1 started only when the download of batch k had ended.)
 int b2z_fetch_small(b200z_ctx* ctx, void* hostDst, const void* d_src, size_t bytes /* multiple of 8, <= 256 */, cudaStream_t st);
+
+// b2z_host_pipeline.cu: the batch pipeline of the host-pointer entry points, over the devices of ctx (ctx, then its peers).  Batch i
+// (srcLen bytes of src at srcOff) goes to worker i mod N, which runs H2D (stream2) | code (stream) | D2H (stream3) over its batches with
+// double-buffered staging: 2 x inStride bytes of dIn, 2 x outStride of dOut.  code(c, i, dIn, dOut, &n) codes batch i on c->stream and
+// synchronises it; its n output bytes go to dst + the sum of the outputs of batches 0 .. i-1, sizes that are known up front (outKnown)
+// or published as the batches are coded.  Returns the first error (a peer's message prefixed with its device), else 0 and *total.
+// No copy from src or into dst is pending when it returns, whatever the exit.
+struct HostBatch { size_t srcOff, srcLen; uint64_t outSize; bool outKnown; };
+using HostCode = std::function<int(b200z_ctx* c, size_t i, const uint8_t* dIn, uint8_t* dOut, uint64_t* out)>;
+int b2z_host_pipeline(b200z_ctx* ctx, const uint8_t* src, uint8_t* dst, const std::vector<HostBatch>& batches, size_t inStride, size_t outStride,
+                      const HostCode& code, uint64_t* total);
 
 // b2z_filter.cu: b200z_filter_device with units -- unitLog != 0 (encode only): the buffer is a run of independent units of 2^unitLog
 // bytes (the xz writer filters every Block on its own)

@@ -5,8 +5,6 @@
 // of it (zstd or skippable) is located by the prepass and decoded in parallel.
 #include "b2z_ctx.h"
 #include <vector>
-#include <thread>
-#include <mutex>
 
 using namespace b2z;
 
@@ -222,9 +220,8 @@ int b200z_zstd_decompress_device(b200z_ctx* ctx, const void* d_src, size_t srcSi
 
 // Host-side split of a compressed stream into batches of whole frames (only when every frame declares its
 // content size): returns false if the stream cannot be split that way (the caller then decodes in one shot).
-struct HostBatch { size_t srcOff, srcEnd; uint64_t dstOff, dstSize; };
 static bool split_frames(const uint8_t* src, size_t srcSize, uint64_t targetOut, std::vector<HostBatch>& out) {
-    size_t ip = 0; HostBatch cur{0, 0, 0, 0}; uint64_t dstPos = 0;
+    size_t ip = 0; HostBatch cur{0, 0, 0, true};
     while (ip < srcSize) {
         if (srcSize - ip < 4) return false;
         const uint32_t magic = rd32(src + ip);
@@ -255,75 +252,16 @@ static bool split_frames(const uint8_t* src, size_t srcSize, uint64_t targetOut,
         }
         if (checksum) { if (srcSize - p < 4) return false; p += 4; }
         ip = p;
-        cur.srcEnd = ip; cur.dstSize += fcs; dstPos += fcs;
-        if (cur.dstSize >= targetOut) { out.push_back(cur); cur = HostBatch{ ip, ip, dstPos, 0 }; }
+        cur.srcLen = ip - cur.srcOff; cur.outSize += fcs;
+        if (cur.outSize >= targetOut) { out.push_back(cur); cur = HostBatch{ ip, 0, 0, true }; }
     }
-    if (cur.srcEnd > cur.srcOff || cur.dstSize) { cur.srcEnd = srcSize; out.push_back(cur); }
-    else if (!out.empty()) out.back().srcEnd = srcSize;
+    if (cur.srcLen || cur.outSize) { cur.srcLen = srcSize - cur.srcOff; out.push_back(cur); }
+    else if (!out.empty()) out.back().srcLen = srcSize - out.back().srcOff;
     return true;
 }
 
-// one device's share of a host-pointer decompress: batches first, first + stride, ... through H2D (stream2) | decode kernels (stream)
-// | D2H (stream3), double-buffered.  Every batch knows where its output goes (the frames declare their sizes), so devices never wait
-// for each other.
-struct DecJob {
-    const uint8_t* src = nullptr; uint8_t* dst = nullptr; const std::vector<HostBatch>* batches = nullptr; size_t inStride = 0, outStride = 0;
-    std::mutex m; int rc = 0; b200z_ctx* errCtx = nullptr;
-    void fail_with(int code, b200z_ctx* c) { std::lock_guard<std::mutex> g(m); if (!rc) { rc = code; errCtx = c; } }
-    bool failed() { std::lock_guard<std::mutex> g(m); return rc != 0; }
-};
-static void dec_worker(b200z_ctx* ctx, DecJob* job, size_t first, size_t stride) {
-    auto run = [&]() -> int {
-        CU(cudaSetDevice(ctx->device));
-        const std::vector<HostBatch>& B = *job->batches;
-        if (ctx->dIn.reserve(2 * job->inStride) || ctx->dOut.reserve(2 * job->outStride)) return fail(ctx, B200Z_E_MEMORY, "device staging allocation failed%s");
-        uint8_t* dIn[2] = { (uint8_t*)ctx->dIn.p, (uint8_t*)ctx->dIn.p + job->inStride };
-        uint8_t* dOut[2] = { (uint8_t*)ctx->dOut.p, (uint8_t*)ctx->dOut.p + job->outStride };
-        // B200Z_TRACE=1: per-batch timeline on stderr (ms since the call began): upload done | kernels begin..end | download done
-        const bool trace = getenv("B200Z_TRACE") != nullptr;
-        std::vector<cudaEvent_t> tev;
-        auto mark = [&](cudaStream_t s) { if (!trace) return; cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s); tev.push_back(e); };
-        mark(ctx->stream2);
-        CU(cudaMemcpyAsync(dIn[0], job->src + B[first].srcOff, B[first].srcEnd - B[first].srcOff, cudaMemcpyHostToDevice, ctx->stream2));
-        CU(cudaEventRecord(ctx->pe[0], ctx->stream2));
-        size_t k = 0;
-        for (size_t i = first; i < B.size(); i += stride, k++) {
-            const int b = (int)(k & 1);
-            if (job->failed()) break;
-            if (i + stride < B.size()) {
-                const HostBatch& nx = B[i + stride];
-                CU(cudaMemcpyAsync(dIn[b ^ 1], job->src + nx.srcOff, nx.srcEnd - nx.srcOff, cudaMemcpyHostToDevice, ctx->stream2));
-                CU(cudaEventRecord(ctx->pe[b ^ 1], ctx->stream2));
-            }
-            CU(cudaStreamWaitEvent(ctx->stream, ctx->pe[b], 0));
-            if (k >= 2) CU(cudaStreamWaitEvent(ctx->stream, ctx->pe[2 + b], 0));
-            mark(ctx->stream);
-            size_t out = 0;
-            int rc = dec_impl(ctx, dIn[b], B[i].srcEnd - B[i].srcOff, dOut[b], (size_t)B[i].dstSize, &out, nullptr);
-            if (rc) return rc;
-            mark(ctx->stream);
-            if (out != B[i].dstSize) return fail(ctx, B200Z_E_CORRUPT, "frame content size mismatch%s");
-            if (out) CU(cudaMemcpyAsync(job->dst + B[i].dstOff, dOut[b], out, cudaMemcpyDeviceToHost, ctx->stream3));
-            CU(cudaEventRecord(ctx->pe[2 + b], ctx->stream3));
-            mark(ctx->stream3);
-            ctx->stat[B200Z_S_H2D_BYTES] += (double)(B[i].srcEnd - B[i].srcOff); ctx->stat[B200Z_S_D2H_BYTES] += (double)out;
-        }
-        CU(cudaStreamSynchronize(ctx->stream3));
-        if (trace) {
-            for (size_t j = 1; j + 2 < tev.size() + 0 && j + 2 <= tev.size() - 0; j += 3) {
-                float a = 0, b2 = 0, c = 0;
-                cudaEventElapsedTime(&a, tev[0], tev[j]); cudaEventElapsedTime(&b2, tev[0], tev[j + 1]); cudaEventElapsedTime(&c, tev[0], tev[j + 2]);
-                fprintf(stderr, "[b200z dec dev %d] batch %zu: kernels %.1f..%.1f  download done %.1f\n", ctx->device, (j - 1) / 3, a, b2, c);
-            }
-            for (cudaEvent_t e : tev) cudaEventDestroy(e);
-        }
-        return 0;
-    };
-    const int rc = run();
-    if (rc) job->fail_with(rc, ctx);
-}
-
-// Host-pointer decompress: batches of whole frames flow through H2D (stream2) | decode kernels (stream) | D2H (stream3).
+// Host-pointer decompress: batches of whole frames flow through the pipeline of b2z_host_pipeline.  Every batch knows where its
+// output goes (the frames declare their sizes), so devices never wait for each other.
 int b200z_zstd_decompress_host(b200z_ctx* ctx, const void* src, size_t srcSize, void* dst, size_t dstCap, size_t* dstSize) {
     if (!ctx || !dstSize || (!src && srcSize) || (!dst && dstCap)) return B200Z_E_PARAM;
     *dstSize = 0;
@@ -345,16 +283,18 @@ int b200z_zstd_decompress_host(b200z_ctx* ctx, const void* src, size_t srcSize, 
         return 0;
     }
     size_t maxIn = 0; uint64_t maxOut = 0, total = 0;
-    for (const HostBatch& b : batches) { if (b.srcEnd - b.srcOff > maxIn) maxIn = b.srcEnd - b.srcOff; if (b.dstSize > maxOut) maxOut = b.dstSize; total += b.dstSize; }
+    for (const HostBatch& b : batches) { if (b.srcLen > maxIn) maxIn = b.srcLen; if (b.outSize > maxOut) maxOut = b.outSize; total += b.outSize; }
     if (total > dstCap) return fail(ctx, B200Z_E_DSTSIZE, "destination too small%s");
-    DecJob job; job.src = (const uint8_t*)src; job.dst = (uint8_t*)dst; job.batches = &batches;
-    job.inStride = (maxIn + 64 + 255) & ~(size_t)255; job.outStride = ((size_t)maxOut + 64 + 255) & ~(size_t)255;
-    const size_t nWorkers = nDev < batches.size() ? nDev : batches.size();
-    std::vector<std::thread> threads;
-    for (size_t d = 1; d < nWorkers; d++) threads.emplace_back(dec_worker, ctx->peers[d - 1], &job, d, nWorkers);
-    dec_worker(ctx, &job, 0, nWorkers);
-    for (std::thread& t : threads) t.join();
-    if (job.rc) { if (job.errCtx && job.errCtx != ctx) snprintf(ctx->err, sizeof(ctx->err), "device %d: %.200s", job.errCtx->device, job.errCtx->err); return job.rc; }
+    const size_t inStride = (maxIn + 64 + 255) & ~(size_t)255, outStride = ((size_t)maxOut + 64 + 255) & ~(size_t)255;
+    const int rc = b2z_host_pipeline(ctx, (const uint8_t*)src, (uint8_t*)dst, batches, inStride, outStride, [&](b200z_ctx* c, size_t i, const uint8_t* dIn, uint8_t* dOut, uint64_t* out) {
+        size_t n = 0;
+        const int drc = dec_impl(c, dIn, batches[i].srcLen, dOut, (size_t)batches[i].outSize, &n, nullptr);
+        if (drc) return drc;
+        if (n != batches[i].outSize) return fail(c, B200Z_E_CORRUPT, "frame content size mismatch%s");
+        *out = n;
+        return 0;
+    }, &total);
+    if (rc) return rc;
     *dstSize = (size_t)total;
     return 0;
 }
