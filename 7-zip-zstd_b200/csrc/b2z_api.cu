@@ -329,8 +329,10 @@ static int enc_batch(b200z_ctx* ctx, const uint8_t* d_src, uint64_t n, uint8_t* 
         launch_lzma2_enc_assemble((const uint8_t*)ctx->slots.p, (const uint32_t*)ctx->slotSize.p, (uint32_t)nChains, (uint32_t)lzma2_enc_slot_stride(g),
                                   (uint64_t*)ctx->frameOff.p, d_dst, (uint64_t*)ctx->scalars.p, st);
     } else {
+        // stage E's records and state words go to the candidate words, which no stage reads after the parse
         launch_zstd_enc_entropy(d_src, n, g, (const uint64_t*)ctx->seqs.p, (const uint32_t*)ctx->nseq.p, (const uint8_t*)ctx->lits.p,
-                                (const uint32_t*)ctx->nlit.p, (uint8_t*)ctx->slots.p, (uint32_t*)ctx->slotSize.p, nBlocks, ctx->smCount, st);
+                                (const uint32_t*)ctx->nlit.p, (uint8_t*)ctx->slots.p, (uint32_t*)ctx->slotSize.p, (uint8_t*)ctx->cand.p,
+                                nBlocks, ctx->smCount, st);
         CU(cudaGetLastError());
         CU(cudaEventRecord(ctx->ev[2], st));
         launch_zstd_enc_assemble(d_src, n, g, (const uint8_t*)ctx->slots.p, (const uint32_t*)ctx->slotSize.p, nBlocks, (uint64_t*)ctx->blockOff.p,

@@ -42,10 +42,12 @@ size_t zstd_enc_parse_smem_bytes();
 cudaError_t launch_zstd_enc_parse(const uint8_t* src, uint64_t srcSize, const EncGeom& g, const uint32_t* cand,
                                   uint64_t* seqs, uint32_t* nseq, uint8_t* lits, uint32_t* nlit, cudaStream_t st);
 
-// stage E: one warp per 128 KiB block -> compressed block (with 3-byte header) in its slot
+// stage E: E1 (tables and literals, one warp per block), E2 (FSE state chains, 30 per warp), E3 (sequence bitstream, one warp
+// per block) -> compressed block (with 3-byte header) in its slot.  scratch: 128 KiB + 3 568 B per block (ENT_SCRATCH_STRIDE),
+// which fits in the 4 bytes per input byte of the candidate words, dead once the parse has run.
 void launch_zstd_enc_entropy(const uint8_t* src, uint64_t srcSize, const EncGeom& g,
                              const uint64_t* seqs, const uint32_t* nseq, const uint8_t* lits, const uint32_t* nlit,
-                             uint8_t* slots, uint32_t* slotSize, uint32_t nBlocks, uint32_t smCount, cudaStream_t st);
+                             uint8_t* slots, uint32_t* slotSize, uint8_t* scratch, uint32_t nBlocks, uint32_t smCount, cudaStream_t st);
 
 // frame assembly: offsets (one CTA scan) + gather of slots into contiguous frames
 void launch_zstd_enc_assemble(const uint8_t* src, uint64_t srcSize, const EncGeom& g, const uint8_t* slots, const uint32_t* slotSize,

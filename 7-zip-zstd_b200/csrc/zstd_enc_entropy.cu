@@ -1,16 +1,18 @@
 // zstd_enc_entropy.cu -- stage E of the block-parallel Zstandard encoder (sm_90a).
 //
-// One WARP compresses one 128 KiB block from stage M's output (final sequences + literal
-// bytes) into a complete zstd block (3-byte header + literals section + sequences section)
-// written to the block's slot.  All 32 lanes cooperate on the data-parallel parts:
-//   - byte histogram of the literals (shared-memory atomics),
-//   - Huffman bit-packing of the 4 literal streams: 32 symbols per iteration, bit offsets by
-//     warp-shuffle prefix sums, codes OR-ed into a shared-memory staging window,
-//   - code histograms of the sequences, and the bit assembly of the sequence stream
-//     (per sequence: three FSE state emissions + LL/ML/OF extra bits).
-// The inherently serial chains run on single lanes while many warps are in flight:
-//   - Huffman tree construction, table descriptions, FSE normalisation/table build (lane 0),
-//   - the three FSE state chains (lanes 0,1,2 -- one per symbol type).
+// Stage E turns stage G's (or stage Z's) output for every 128 KiB block -- final sequences + literal bytes -- into a complete
+// zstd block (3-byte header + literals section + sequences section) in the block's slot.  It runs as three kernels:
+//   E1 (zstd_enc_tables_kernel, one warp per block): RLE-block test, literal histogram, Huffman code and description, the
+//      whole literals section (with the raw and RLE fallbacks), the code histograms, the three mode/table choices, NCount
+//      headers, the sequence-section header and the size bound.  The table work is warp-wide: present symbols ranked by
+//      compares, one symbol per lane for normalisation and costs, the FSE spread numbered by ballots, the state fill
+//      ranked by __match_any_sync.  Blocks that need no FSE chain (RLE blocks, no sequences, over the bound) are finished
+//      here; every other block leaves an EntRec (header sizes, logs, the three encoding tables) in scratch.
+//   E2 (zstd_enc_chains_kernel, 30 chains per warp): lane 3b+t runs the FSE state chain of symbol type t (LL, OF, ML) of
+//      block b of the warp's 10; the three lanes of a block step together from the last sequence to the first and leave
+//      one 32-bit word per sequence: the three states' bits in stream order (OF, ML, LL; <= 26 bits) and their count.
+//   E3 (zstd_enc_seqbits_kernel, one warp per block): the sequence bitstream -- state word + LL/ML/OF extra bits per
+//      sequence, placed by prefix sum -- then the final states, the end mark, and the compressed-or-raw block choice.
 //
 // Replaces (reference, /root/reference/C/zstd/): zstd_compress.c:2888
 // (ZSTD_entropyCompressSeqStore_internal), zstd_compress_literals.c:129-235, hist.c:164,
@@ -62,7 +64,16 @@ __device__ __forceinline__ uint32_t ml_code(uint32_t m) {   // m = matchLength -
     return highbit32(m) + 36;
 }
 
-// ---------------------------------------------------------------- per-warp workspace
+__device__ __forceinline__ uint32_t warp_sum(uint32_t v) {
+    for (int d = 16; d; d >>= 1) v += __shfl_xor_sync(B2Z_FULL, v, d);
+    return v;
+}
+__device__ __forceinline__ uint32_t warp_max(uint32_t v) {
+    for (int d = 16; d; d >>= 1) { const uint32_t o = __shfl_xor_sync(B2Z_FULL, v, d); v = o > v ? o : v; }
+    return v;
+}
+
+// ---------------------------------------------------------------- per-warp workspace of E1
 struct FseCT {                       // FSE encoding table of one symbol type
     uint16_t state[512];
     int32_t  dfs[64];                // deltaFindState
@@ -78,16 +89,44 @@ struct WarpWS {
     uint16_t hufCode[256];
     uint8_t  hufLen[256];
     union {
-        struct { uint32_t w[512]; uint16_t parent[512]; uint8_t order[256]; uint8_t depth[512]; } hb;   // Huffman build
-        struct { FseCT ct[3]; } fse;                                                                      // LL, OF, ML
+        struct { uint32_t w[512]; uint16_t parent[512]; uint8_t order[256]; uint8_t depth[512]; uint32_t key[256]; } hb;   // Huffman build
+        struct { FseCT ct[3]; } fse;                                                                                        // LL, OF, ML
     } u;
     uint8_t  spread[512];            // FSE symbol spreading scratch
     int16_t  norm[64];
+    uint16_t cumul[66];              // FSE build: first state slot of each symbol, then its running fill position
+    uint16_t cpos[66];               // FSE build: first spread index of each symbol with a positive count
+    uint32_t rk[16], rstart[16], rnext[16];   // Huffman canonical codes: symbols per rank, first code, codes given so far
+    uint32_t wcnt[16];               // Huffman weight counts
     uint32_t stage[STAGE_WORDS];     // bit staging window
-    uint8_t  bcode[3][32];           // per-batch codes (LL, OF, ML)
-    uint16_t bbits[3][32];           // per-batch FSE state bits
-    uint8_t  bnb[3][32];
 };
+
+// ---------------------------------------------------------------- E1 -> E2 -> E3 record, one per block in scratch
+// The three encoding tables in the layout E2 keeps in shared memory: states LL | OF | ML, then {deltaNbBits, deltaFindState}
+// per symbol LL | OF | ML.
+#define ENT_ST_OF 512u
+#define ENT_ST_ML 768u
+#define ENT_ST_N  1280u
+#define ENT_SY_OF 36u
+#define ENT_SY_ML 68u
+#define ENT_SY_N  121u
+struct EntTables {
+    uint16_t state[ENT_ST_N];
+    uint2    sym[ENT_SY_N];
+    uint32_t pad[2];
+};
+struct EntRec {
+    uint32_t run;                    // 1: E2 and E3 code this block's sequences; 0: E1 finished the block
+    uint32_t bodyHead;               // bytes of the block body before the sequence bitstream
+    uint32_t logs;                   // table logs: LL | OF << 8 | ML << 16
+    uint32_t pad0;
+    uint16_t fin[4];                 // final states LL, OF, ML (written by E2)
+    uint32_t pad1[2];
+    EntTables tab;
+};
+static_assert(sizeof(EntTables) % 16 == 0 && sizeof(EntRec) % 16 == 0 && offsetof(EntRec, tab) % 16 == 0, "EntRec is copied in 16-byte units");
+#define ENT_SCRATCH_STRIDE ((size_t)sizeof(EntRec) + (size_t)B2Z_MAXSEQ * 4u)   // record, then one state word per sequence
+static_assert(sizeof(EntRec) + (size_t)B2Z_MAXSEQ * 4u <= (size_t)B2Z_BLOCK * 4u, "stage E scratch must fit the block's candidate words");
 
 // ---------------------------------------------------------------- lane-0 bit writer to global memory
 struct BitW {
@@ -101,31 +140,62 @@ struct BitW {
     __device__ __forceinline__ uint8_t* flush_partial() { if (nb) { *p++ = (uint8_t)acc; acc = 0; nb = 0; } return p; }
 };
 
-// ---------------------------------------------------------------- FSE (lane 0)
-__device__ void fse_build_ctable(FseCT* ct, uint8_t* spread, const int16_t* norm, uint32_t maxSym, uint32_t log) {
-    const uint32_t size = 1u << log, mask = size - 1u, step = (size >> 1) + (size >> 3) + 3u;
-    uint32_t cumul[65], high = size - 1u;
-    cumul[0] = 0;
-    for (uint32_t s = 0; s <= maxSym; s++) {
-        if (norm[s] == -1) { cumul[s + 1] = cumul[s] + 1u; spread[high--] = (uint8_t)s; }
-        else cumul[s + 1] = cumul[s] + (uint32_t)norm[s];
-    }
-    uint32_t pos = 0;
-    for (uint32_t s = 0; s <= maxSym; s++)
-        for (int i = 0; i < norm[s]; i++) { spread[pos] = (uint8_t)s; pos = (pos + step) & mask; while (pos > high) pos = (pos + step) & mask; }
-    for (uint32_t u = 0; u < size; u++) { const uint32_t s = spread[u]; ct->state[cumul[s]++] = (uint16_t)(size + u); }
-    uint32_t total = 0;
-    for (uint32_t s = 0; s <= maxSym; s++) {
-        const int n = norm[s];
-        if (n == 0) { ct->dnb[s] = ((log + 1u) << 16) - size; ct->dfs[s] = 0; }
-        else if (n == 1 || n == -1) { ct->dnb[s] = (log << 16) - size; ct->dfs[s] = (int32_t)total - 1; total++; }
-        else {
-            const uint32_t maxBitsOut = log - highbit32((uint32_t)n - 1u), minStatePlus = (uint32_t)n << maxBitsOut;
-            ct->dnb[s] = (maxBitsOut << 16) - minStatePlus;
-            ct->dfs[s] = (int32_t)total - n; total += (uint32_t)n;
+// ---------------------------------------------------------------- FSE (warp-wide unless noted)
+// Encoding table of `norm` (symbols 0..maxSym, maxSym < 64, log >= 5).  The serial statement spreads the symbols in order
+// over positions k*step & mask (k = 0, 1, ...), skipping those above `high` where the "less than 1" symbols sit; step is odd,
+// so every position is visited once, and the m-th accepted position takes the m-th slot of the symbols' count runs.
+__device__ void fse_build_ctable(WarpWS* ws, FseCT* ct, const int16_t* norm, uint32_t maxSym, uint32_t log, uint32_t lane) {
+    const uint32_t size = 1u << log, mask = size - 1u, step = (size >> 1) + (size >> 3) + 3u, lt = (1u << lane) - 1u;
+    uint16_t* cumul = ws->cumul; uint16_t* cpos = ws->cpos; uint8_t* spread = ws->spread;
+    uint32_t cu = 0, cp = 0, nLow = 0;
+    for (uint32_t s0 = 0; s0 <= maxSym; s0 += 32) {
+        const uint32_t s = s0 + lane;
+        const int n = s <= maxSym ? norm[s] : 0;
+        uint32_t tc, tp;
+        const uint32_t ec = warp_excl_scan(n == -1 ? 1u : (n > 0 ? (uint32_t)n : 0u), lane, &tc);
+        const uint32_t ep = warp_excl_scan(n > 0 ? (uint32_t)n : 0u, lane, &tp);
+        const uint32_t low = __ballot_sync(B2Z_FULL, n == -1);
+        if (s <= maxSym) {
+            const uint32_t total = cu + ec;
+            cumul[s] = (uint16_t)total; cpos[s] = (uint16_t)(cp + ep);
+            if (n == 0) { ct->dnb[s] = ((log + 1u) << 16) - size; ct->dfs[s] = 0; }
+            else if (n == 1 || n == -1) { ct->dnb[s] = (log << 16) - size; ct->dfs[s] = (int32_t)total - 1; }
+            else {
+                const uint32_t maxBitsOut = log - highbit32((uint32_t)n - 1u), minStatePlus = (uint32_t)n << maxBitsOut;
+                ct->dnb[s] = (maxBitsOut << 16) - minStatePlus;
+                ct->dfs[s] = (int32_t)total - n;
+            }
+            if (n == -1) spread[size - 1u - nLow - (uint32_t)__popc(low & lt)] = (uint8_t)s;
         }
+        cu += tc; cp += tp; nLow += (uint32_t)__popc(low);
     }
-    ct->log = log;
+    __syncwarp();
+    const uint32_t high = size - 1u - nLow;
+    uint32_t m0 = 0;
+    for (uint32_t k0 = 0; k0 < size; k0 += 32) {
+        const uint32_t k = k0 + lane, pos = (k * step) & mask;
+        const bool acc = k < size && pos <= high;
+        const uint32_t bal = __ballot_sync(B2Z_FULL, acc);
+        if (acc) {
+            const uint32_t m = m0 + (uint32_t)__popc(bal & lt);
+            uint32_t lo = 0, hi = maxSym + 1u;                   // the last symbol whose run starts at or before m
+            while (hi - lo > 1u) { const uint32_t mid = (lo + hi) >> 1; if (cpos[mid] <= m) lo = mid; else hi = mid; }
+            spread[pos] = (uint8_t)lo;
+        }
+        m0 += (uint32_t)__popc(bal);
+    }
+    __syncwarp();
+    for (uint32_t u0 = 0; u0 < size; u0 += 32) {                 // state fill in spread order, per symbol
+        const uint32_t u = u0 + lane;
+        const uint32_t s = u < size ? spread[u] : 0xFFFFu;
+        const uint32_t grp = __match_any_sync(B2Z_FULL, s);
+        if (u < size) ct->state[cumul[s] + (uint32_t)__popc(grp & lt)] = (uint16_t)(size + u);
+        __syncwarp();
+        if (u < size && (grp >> lane) == 1u) cumul[s] = (uint16_t)(cumul[s] + __popc(grp));
+        __syncwarp();
+    }
+    if (lane == 0) ct->log = log;
+    __syncwarp();
 }
 __device__ __forceinline__ uint32_t fse_init_state(const FseCT* ct, uint32_t sym) {
     const uint32_t nb = (ct->dnb[sym] + (1u << 15)) >> 16;
@@ -138,27 +208,39 @@ __device__ __forceinline__ uint32_t fse_encode(const FseCT* ct, uint32_t* state,
     *nbOut = nb; return bits;
 }
 
-__device__ void fse_normalize(int16_t* norm, uint32_t log, const uint32_t* count, uint32_t total, uint32_t maxSym) {
-    const uint32_t size = 1u << log; int32_t sum = 0;
-    for (uint32_t s = 0; s <= maxSym; s++) {
-        if (!count[s]) { norm[s] = 0; continue; }
-        uint64_t p = ((uint64_t)count[s] * size * 2u + total) / (2ull * total);
-        if (p < 1) p = 1;
-        norm[s] = (int16_t)p; sum += (int32_t)p;
-    }
-    int32_t delta = (int32_t)size - sum;
-    while (delta != 0) {
-        uint32_t big = 0;
-        for (uint32_t s = 1; s <= maxSym; s++) if (norm[s] > norm[big]) big = s;
-        if (delta > 0) { norm[big] = (int16_t)(norm[big] + delta); delta = 0; }
-        else {
-            int32_t take = norm[big] - 1 < -delta ? norm[big] - 1 : -delta;
-            if (take > (norm[big] >> 1) && norm[big] > 2) take = norm[big] >> 1;
-            norm[big] = (int16_t)(norm[big] - take); delta += take;
+// rounding one symbol per lane, then the settle loop on the (first) largest entry
+__device__ void fse_normalize(int16_t* norm, uint32_t log, const uint32_t* count, uint32_t total, uint32_t maxSym, uint32_t lane) {
+    const uint32_t size = 1u << log; uint32_t sum = 0;
+    for (uint32_t s = lane; s <= maxSym; s += 32) {
+        int16_t v = 0;
+        if (count[s]) {
+            uint64_t p = ((uint64_t)count[s] * size * 2u + total) / (2ull * total);
+            if (p < 1) p = 1;
+            v = (int16_t)p; sum += (uint32_t)p;
         }
+        norm[s] = v;
+    }
+    int32_t delta = (int32_t)size - (int32_t)warp_sum(sum);
+    __syncwarp();
+    while (delta != 0) {
+        uint32_t key = 0;                                        // (entry, lowest index first)
+        for (uint32_t s = lane; s <= maxSym; s += 32) { const uint32_t k = ((uint32_t)norm[s] << 8) | (255u - s); key = k > key ? k : key; }
+        key = warp_max(key);
+        const uint32_t big = 255u - (key & 255u); const int32_t nbig = (int32_t)(key >> 8);
+        int32_t nv;
+        if (delta > 0) { nv = nbig + delta; delta = 0; }
+        else {
+            int32_t take = nbig - 1 < -delta ? nbig - 1 : -delta;
+            if (take > (nbig >> 1) && nbig > 2) take = nbig >> 1;
+            nv = nbig - take; delta += take;
+        }
+        __syncwarp();
+        if (lane == 0) norm[big] = (int16_t)nv;
+        __syncwarp();
     }
 }
 
+// lane 0
 __device__ uint32_t fse_write_ncount(uint8_t* dst, const int16_t* norm, uint32_t maxSym, uint32_t log) {
     BitW b; b.init(dst);
     b.add(log - 5u, 4);
@@ -190,74 +272,105 @@ __device__ __forceinline__ uint32_t log2_fx8(uint32_t x) {
     const uint32_t m = hb >= 5 ? (x >> (hb - 5)) & 31u : (x << (5 - hb)) & 31u;
     return (hb << 8) + d_log2frac[m];
 }
-__device__ uint64_t fse_cost_fx8(const uint32_t* count, const int16_t* norm, uint32_t maxSym, uint32_t log) {
-    uint64_t c = 0;
-    for (uint32_t s = 0; s <= maxSym; s++) {
+__device__ uint64_t fse_cost_fx8(const uint32_t* count, const int16_t* norm, uint32_t maxSym, uint32_t log, uint32_t lane) {
+    uint64_t c = 0; bool bad = false;
+    for (uint32_t s = lane; s <= maxSym; s += 32) {
         if (!count[s]) continue;
-        if (norm[s] == 0) return ~0ull;
+        if (norm[s] == 0) { bad = true; continue; }
         const uint32_t n = norm[s] < 0 ? 1u : (uint32_t)norm[s];
         c += (uint64_t)count[s] * ((log << 8) - log2_fx8(n));
     }
+    if (__any_sync(B2Z_FULL, bad)) return ~0ull;
+    for (int d = 16; d; d >>= 1) c += __shfl_xor_sync(B2Z_FULL, c, d);
     return c;
 }
 
-// ---------------------------------------------------------------- Huffman (lane 0)
+// ---------------------------------------------------------------- Huffman (warp-wide; the tree itself on lane 0)
 // code lengths (<= 11) into ws->hufLen / hufCode; returns maxBits, sets *maxSymOut
-__device__ uint32_t huf_build(WarpWS* ws, uint32_t* maxSymOut) {
-    uint32_t* count = ws->hist;
+__device__ uint32_t huf_build(WarpWS* ws, uint32_t lane, uint32_t* maxSymOut) {
+    const uint32_t* count = ws->hist;
     uint32_t* w = ws->u.hb.w; uint16_t* parent = ws->u.hb.parent; uint8_t* order = ws->u.hb.order; uint8_t* depth = ws->u.hb.depth;
+    uint32_t* key = ws->u.hb.key;
+    const uint32_t lt = (1u << lane) - 1u;
     uint32_t n, maxd;
-#define EFFC(s) ((count[s] + (1u << k) - 1u) >> k)          /* count after k halvings (ceil) */
     for (uint32_t k = 0;; k++) {
+        // present symbols keyed by (count after k halvings, rounded up; symbol); the rank of a key among them is its place
+        // in the stable sort by count
         n = 0;
-        for (uint32_t s = 0; s < 256; s++) if (count[s]) order[n++] = (uint8_t)s;
-        for (uint32_t i = 1; i < n; i++) {                       // stable insertion sort by count
-            const uint32_t s = order[i], c = EFFC(s); int j = (int)i - 1;
-            while (j >= 0 && EFFC(order[j]) > c) { order[j + 1] = order[j]; j--; }
-            order[j + 1] = (uint8_t)s;
+        for (uint32_t s0 = 0; s0 < 256; s0 += 32) {
+            const uint32_t s = s0 + lane, c = count[s];
+            const uint32_t bal = __ballot_sync(B2Z_FULL, c != 0);
+            if (c) key[n + (uint32_t)__popc(bal & lt)] = (((c + (1u << k) - 1u) >> k) << 8) | s;
+            n += (uint32_t)__popc(bal);
         }
-        for (uint32_t i = 0; i < n; i++) w[i] = EFFC(order[i]);
-        uint32_t li = 0, ii = n, ie = n;
-        while ((n - li) + (ie - ii) > 1) {
-            uint32_t a, b;
-            if (li < n && (ii >= ie || w[li] <= w[ii])) a = li++; else a = ii++;
-            if (li < n && (ii >= ie || w[li] <= w[ii])) b = li++; else b = ii++;
-            w[ie] = w[a] + w[b]; parent[a] = (uint16_t)ie; parent[b] = (uint16_t)ie; ie++;
+        __syncwarp();
+        for (uint32_t i = lane; i < n; i += 32) {
+            const uint32_t ki = key[i]; uint32_t r = 0;
+            for (uint32_t j = 0; j < n; j++) r += key[j] < ki ? 1u : 0u;
+            order[r] = (uint8_t)ki; w[r] = ki >> 8;
         }
-        maxd = 0; depth[ie - 1] = 0;
-        for (int i = (int)ie - 2; i >= 0; i--) depth[i] = (uint8_t)(depth[parent[i]] + 1);
-        for (uint32_t i = 0; i < n; i++) if (depth[i] > maxd) maxd = depth[i];
+        __syncwarp();
+        uint32_t md = 0;
+        if (lane == 0) {                                         // two-queue tree on the sorted weights
+            uint32_t li = 0, ii = n, ie = n;
+            while ((n - li) + (ie - ii) > 1) {
+                uint32_t a, b;
+                if (li < n && (ii >= ie || w[li] <= w[ii])) a = li++; else a = ii++;
+                if (li < n && (ii >= ie || w[li] <= w[ii])) b = li++; else b = ii++;
+                w[ie] = w[a] + w[b]; parent[a] = (uint16_t)ie; parent[b] = (uint16_t)ie; ie++;
+            }
+            depth[ie - 1] = 0;
+            for (int i = (int)ie - 2; i >= 0; i--) depth[i] = (uint8_t)(depth[parent[i]] + 1);
+            for (uint32_t i = 0; i < n; i++) if (depth[i] > md) md = depth[i];
+        }
+        maxd = __shfl_sync(B2Z_FULL, md, 0);
+        __syncwarp();
         if (maxd <= 11) break;
     }
-#undef EFFC
-    for (uint32_t s = 0; s < 256; s++) ws->hufLen[s] = 0;
-    for (uint32_t i = 0; i < n; i++) ws->hufLen[order[i]] = depth[i];
+    for (uint32_t s = lane; s < 256; s += 32) ws->hufLen[s] = 0;
+    if (lane < 16) { ws->rk[lane] = 0; ws->rnext[lane] = 0; }
+    __syncwarp();
+    for (uint32_t i = lane; i < n; i += 32) ws->hufLen[order[i]] = depth[i];
+    __syncwarp();
     uint32_t maxSym = 0;
-    for (uint32_t s = 0; s < 256; s++) if (count[s]) maxSym = s;
-    uint32_t rank[13], start[13], pos = 0;
-    for (uint32_t r = 0; r < 13; r++) rank[r] = 0;
-    for (uint32_t s = 0; s < 256; s++) if (ws->hufLen[s]) rank[maxd + 1u - ws->hufLen[s]]++;
-    for (uint32_t r = 1; r <= maxd; r++) { start[r] = pos; pos += rank[r] << (r - 1u); }
-    for (uint32_t s = 0; s < 256; s++) {
-        if (!ws->hufLen[s]) { ws->hufCode[s] = 0; continue; }
-        const uint32_t r = maxd + 1u - ws->hufLen[s];
-        ws->hufCode[s] = (uint16_t)(start[r] >> (r - 1u)); start[r] += 1u << (r - 1u);
+    for (uint32_t s = lane; s < 256; s += 32) {
+        if (count[s]) maxSym = s;
+        if (ws->hufLen[s]) atomicAdd(&ws->rk[maxd + 1u - ws->hufLen[s]], 1u);
+    }
+    maxSym = warp_max(maxSym);
+    __syncwarp();
+    if (lane == 0) { uint32_t pos = 0; for (uint32_t r = 1; r <= maxd; r++) { ws->rstart[r] = pos; pos += ws->rk[r] << (r - 1u); } }
+    __syncwarp();
+    // canonical codes: within a rank, in symbol order
+    for (uint32_t s0 = 0; s0 < 256; s0 += 32) {
+        const uint32_t s = s0 + lane, len = ws->hufLen[s], r = len ? maxd + 1u - len : 0u;
+        const uint32_t grp = __match_any_sync(B2Z_FULL, r);
+        ws->hufCode[s] = len ? (uint16_t)((ws->rstart[r] >> (r - 1u)) + ws->rnext[r] + (uint32_t)__popc(grp & lt)) : (uint16_t)0;
+        __syncwarp();
+        if (len && (grp >> lane) == 1u) ws->rnext[r] += (uint32_t)__popc(grp);
+        __syncwarp();
     }
     *maxSymOut = maxSym;
     return maxd;
 }
 
 // tree description at dst; returns bytes written or 0 (not representable)
-__device__ uint32_t huf_write_table(WarpWS* ws, uint8_t* dst, uint32_t maxBits, uint32_t maxSym) {
+__device__ uint32_t huf_write_table(WarpWS* ws, uint8_t* dst, uint32_t maxBits, uint32_t maxSym, uint32_t lane) {
     const uint32_t nw = maxSym;
     uint8_t* wt = ws->u.hb.order;                                // weights (hb scratch is dead now; order[256] reused)
-    for (uint32_t s = 0; s < nw; s++) wt[s] = ws->hufLen[s] ? (uint8_t)(maxBits + 1u - ws->hufLen[s]) : 0;
+    uint32_t maxW = 0;
+    for (uint32_t s = lane; s < nw; s += 32) {
+        const uint32_t v = ws->hufLen[s] ? maxBits + 1u - ws->hufLen[s] : 0u;
+        wt[s] = (uint8_t)v; maxW = v > maxW ? v : maxW;
+    }
+    maxW = warp_max(maxW);
+    if (lane < 16) ws->wcnt[lane] = 0;
+    __syncwarp();
     uint32_t fseSize = 0;
     if (nw > 1) {
-        uint32_t cnt[16], maxW = 0, maxCnt = 0;
-        for (uint32_t i = 0; i < 16; i++) cnt[i] = 0;
-        for (uint32_t i = 0; i < nw; i++) { cnt[wt[i]]++; if (wt[i] > maxW) maxW = wt[i]; }
-        for (uint32_t i = 0; i <= maxW; i++) if (cnt[i] > maxCnt) maxCnt = cnt[i];
+        for (uint32_t s = lane; s < nw; s += 32) atomicAdd(&ws->wcnt[wt[s]], 1u);
+        __syncwarp();
+        const uint32_t maxCnt = warp_max(lane <= maxW ? ws->wcnt[lane] : 0u);
         if (maxCnt != nw && maxCnt > 1) {
             uint32_t log = 6;
             const uint32_t minBits = highbit32(nw) + 1u, symBits = highbit32(maxW + 1u) + 2u;
@@ -268,33 +381,38 @@ __device__ uint32_t huf_write_table(WarpWS* ws, uint8_t* dst, uint32_t maxBits, 
             if (log < 5) log = 5;
             if (log > 6) log = 6;
             int16_t* norm = ws->norm;
-            fse_normalize(norm, log, cnt, nw, maxW);
+            fse_normalize(norm, log, ws->wcnt, nw, maxW, lane);
             uint8_t* tmp = dst + 1;
-            const uint32_t hs = fse_write_ncount(tmp, norm, maxW, log);
-            // weights table: a 64-state FseCT carved out of the stage buffer (unused at this point)
-            FseCT* ct = reinterpret_cast<FseCT*>(ws->u.hb.w);    // hb.w (2 KiB) + parent: large enough for FseCT? see static_assert
-            fse_build_ctable(ct, ws->spread, norm, maxW, log);
-            BitW b; b.init(tmp + hs);
-            uint32_t i = nw, s1, s2, nb, bits;
-            if (nw & 1u) { s1 = fse_init_state(ct, wt[--i]); s2 = fse_init_state(ct, wt[--i]);
-                           bits = fse_encode(ct, &s1, wt[--i], &nb); b.add(bits, nb); }
-            else { s2 = fse_init_state(ct, wt[--i]); s1 = fse_init_state(ct, wt[--i]); }
-            while (i > 0) {
-                bits = fse_encode(ct, &s2, wt[--i], &nb); b.add(bits, nb);
-                bits = fse_encode(ct, &s1, wt[--i], &nb); b.add(bits, nb);
+            uint32_t hs = 0;
+            if (lane == 0) hs = fse_write_ncount(tmp, norm, maxW, log);
+            hs = __shfl_sync(B2Z_FULL, hs, 0);
+            // weights table: a 64-state FseCT carved out of hb.w (dead at this point)
+            FseCT* ct = reinterpret_cast<FseCT*>(ws->u.hb.w);
+            fse_build_ctable(ws, ct, norm, maxW, log, lane);
+            if (lane == 0) {
+                BitW b; b.init(tmp + hs);
+                uint32_t i = nw, s1, s2, nb, bits;
+                if (nw & 1u) { s1 = fse_init_state(ct, wt[--i]); s2 = fse_init_state(ct, wt[--i]);
+                               bits = fse_encode(ct, &s1, wt[--i], &nb); b.add(bits, nb); }
+                else { s2 = fse_init_state(ct, wt[--i]); s1 = fse_init_state(ct, wt[--i]); }
+                while (i > 0) {
+                    bits = fse_encode(ct, &s2, wt[--i], &nb); b.add(bits, nb);
+                    bits = fse_encode(ct, &s1, wt[--i], &nb); b.add(bits, nb);
+                }
+                b.add(s2, log); b.add(s1, log);
+                fseSize = (uint32_t)(b.close() - tmp);
             }
-            b.add(s2, log); b.add(s1, log);
-            fseSize = (uint32_t)(b.close() - tmp);
+            fseSize = __shfl_sync(B2Z_FULL, fseSize, 0);
         }
     }
     const uint32_t rawSize = (nw + 1u) / 2u;
-    if (fseSize && fseSize < 128u && (fseSize < rawSize || nw > 128u)) { dst[0] = (uint8_t)fseSize; return 1u + fseSize; }
+    if (fseSize && fseSize < 128u && (fseSize < rawSize || nw > 128u)) { if (lane == 0) dst[0] = (uint8_t)fseSize; return 1u + fseSize; }
     if (nw > 128u || nw == 0u) return 0;
-    dst[0] = (uint8_t)(127u + nw);
-    for (uint32_t i = 0; i < nw; i += 2) dst[1 + i / 2] = (uint8_t)((wt[i] << 4) | (i + 1 < nw ? wt[i + 1] : 0));
+    if (lane == 0) dst[0] = (uint8_t)(127u + nw);
+    for (uint32_t i = 2u * lane; i < nw; i += 64) dst[1 + i / 2] = (uint8_t)((wt[i] << 4) | (i + 1 < nw ? wt[i + 1] : 0));
     return 1u + rawSize;
 }
-static_assert(sizeof(FseCT) <= sizeof(uint32_t) * 512 + sizeof(uint16_t) * 512, "weights FseCT must fit in hb.w+hb.parent");
+static_assert(sizeof(FseCT) <= sizeof(uint32_t) * 512, "weights FseCT must fit in hb.w");
 
 // ---------------------------------------------------------------- warp bit staging
 struct Stager {
@@ -330,13 +448,17 @@ struct Stager {
     }
 };
 
-// Huffman-encode literals [a, b) as one backward stream at st.out; returns stream bytes
+// Huffman-encode literals [a, b) as one backward stream at st.out, 4 literals per lane and 128 per step; returns stream bytes
 __device__ uint32_t huf_encode_stream(WarpWS* ws, Stager& st, const uint8_t* __restrict__ lit, uint32_t a, uint32_t b, uint32_t lane) {
     uint8_t* start = st.out;
     for (uint32_t hi = b; hi > a;) {
-        const uint32_t cnt = (hi - a) < 32u ? (hi - a) : 32u;
-        uint32_t code = 0, nb = 0;
-        if (lane < cnt) { const uint32_t s = lit[hi - 1u - lane]; code = ws->hufCode[s]; nb = ws->hufLen[s]; }
+        const uint32_t cnt = (hi - a) < 128u ? (hi - a) : 128u;
+        uint64_t code = 0; uint32_t nb = 0;                      // lane's literals hi-1-4*lane .. hi-4-4*lane, <= 44 bits
+#pragma unroll
+        for (uint32_t j = 0; j < 4; j++) {
+            const uint32_t k = lane * 4u + j;
+            if (k < cnt) { const uint32_t s = lit[hi - 1u - k]; code |= (uint64_t)ws->hufCode[s] << nb; nb += ws->hufLen[s]; }
+        }
         uint32_t total; const uint32_t off = warp_excl_scan(nb, lane, &total);
         st.put(st.bits + off, code, 0, nb);
         st.bits += total; hi -= cnt;
@@ -352,21 +474,29 @@ __device__ __forceinline__ void warp_copy(uint8_t* dst, const uint8_t* __restric
     for (uint32_t i = lane; i < n; i += 32) dst[i] = src[i];
 }
 
-// ---------------------------------------------------------------- sequence table choice (lane 0)
+// ---------------------------------------------------------------- sequence table choice (warp-wide)
 // returns header bytes written at dst; *mode = 0 predefined, 1 RLE, 2 compressed
 __device__ uint32_t choose_seq_table(WarpWS* ws, FseCT* ct, uint8_t* dst, const uint32_t* count, uint32_t nbSeq, uint32_t maxSymAll,
-                                     uint32_t maxLog, const int16_t* defNorm, uint32_t defMaxSym, uint32_t defLog, uint32_t* mode) {
+                                     uint32_t maxLog, const int16_t* defNorm, uint32_t defMaxSym, uint32_t defLog, uint32_t* mode, uint32_t lane) {
     uint32_t maxSym = 0, present = 0, big = 0;
-    for (uint32_t s = 0; s <= maxSymAll; s++) if (count[s]) { maxSym = s; present++; if (count[s] > big) big = count[s]; }
+    for (uint32_t s = lane; s <= maxSymAll; s += 32) if (count[s]) { maxSym = s; present++; if (count[s] > big) big = count[s]; }
+    maxSym = warp_max(maxSym); present = warp_sum(present); big = warp_max(big);
     if (big == nbSeq && !(nbSeq <= 2 && maxSym <= defMaxSym)) {
-        for (uint32_t s = 0; s < 64; s++) { ct->dnb[s] = 0; ct->dfs[s] = 0; }
-        ct->state[0] = 0; ct->state[1] = 0; ct->log = 0;
-        *mode = 1; dst[0] = (uint8_t)maxSym; return 1;
+        for (uint32_t s = lane; s < 64; s += 32) { ct->dnb[s] = 0; ct->dfs[s] = 0; }
+        if (lane < 2) ct->state[lane] = 0;
+        if (lane == 0) { ct->log = 0; dst[0] = (uint8_t)maxSym; }
+        __syncwarp();
+        *mode = 1; return 1;
     }
     int16_t* norm = ws->norm;
     // default-table cost (copy default norm into smem for the shared cost routine)
     uint64_t costDef = ~0ull;
-    if (maxSym <= defMaxSym) { for (uint32_t s = 0; s <= defMaxSym; s++) norm[s] = defNorm[s]; costDef = fse_cost_fx8(count, norm, maxSym, defLog); }
+    if (maxSym <= defMaxSym) {
+        for (uint32_t s = lane; s <= defMaxSym; s += 32) norm[s] = defNorm[s];
+        __syncwarp();
+        costDef = fse_cost_fx8(count, norm, maxSym, defLog, lane);
+        __syncwarp();
+    }
     const uint32_t hbN = highbit32(nbSeq > 1 ? nbSeq - 1u : 1u);
     uint32_t log = hbN >= 2 ? hbN - 2u : 0u;
     const uint32_t minA = highbit32(nbSeq) + 1u, minB = highbit32(maxSym ? maxSym : 1u) + 2u, lo = minA < minB ? minA : minB;
@@ -375,41 +505,67 @@ __device__ uint32_t choose_seq_table(WarpWS* ws, FseCT* ct, uint8_t* dst, const 
     if (log < 5) log = 5;
     if (log > maxLog) log = maxLog;
     while ((1u << log) < present) log++;
-    fse_normalize(norm, log, count, nbSeq, maxSym);
-    const uint32_t hs = fse_write_ncount(dst, norm, maxSym, log);
-    const uint64_t costFse = fse_cost_fx8(count, norm, maxSym, log) + ((uint64_t)hs << 11);
+    fse_normalize(norm, log, count, nbSeq, maxSym, lane);
+    uint32_t hs = 0;
+    if (lane == 0) hs = fse_write_ncount(dst, norm, maxSym, log);
+    hs = __shfl_sync(B2Z_FULL, hs, 0);
+    const uint64_t costFse = fse_cost_fx8(count, norm, maxSym, log, lane) + ((uint64_t)hs << 11);
+    __syncwarp();
     if (costDef <= costFse || big == nbSeq) {
-        for (uint32_t s = 0; s <= defMaxSym; s++) norm[s] = defNorm[s];
-        fse_build_ctable(ct, ws->spread, norm, defMaxSym, defLog); *mode = 0; return 0;
+        for (uint32_t s = lane; s <= defMaxSym; s += 32) norm[s] = defNorm[s];
+        __syncwarp();
+        fse_build_ctable(ws, ct, norm, defMaxSym, defLog, lane); *mode = 0; return 0;
     }
-    fse_build_ctable(ct, ws->spread, norm, maxSym, log); *mode = 2; return hs;
+    fse_build_ctable(ws, ct, norm, maxSym, log, lane); *mode = 2; return hs;
 }
 
-// ---------------------------------------------------------------- the kernel
+// ---------------------------------------------------------------- block geometry
+struct BlockGeom { uint32_t blkSize, last; size_t litOff; };   // litOff: the block's offset in the source and literal buffers
+__device__ __forceinline__ BlockGeom block_geom(const EncGeom& g, uint64_t srcSize, uint32_t blk) {
+    const uint32_t blocksPerFrame = 1u << (g.frameLog - 17u);
+    const uint64_t frame = blk / blocksPerFrame; const uint32_t bif = blk % blocksPerFrame;
+    const uint64_t f0 = frame << g.frameLog;
+    const uint64_t fn = enc_frame_bytes(g, srcSize, frame);
+    const uint64_t b0 = (uint64_t)bif << 17;
+    BlockGeom r;
+    r.blkSize = (uint32_t)((fn - b0) < B2Z_BLOCK ? (fn - b0) : B2Z_BLOCK);
+    r.last = (b0 + r.blkSize == fn) ? 1u : 0u;
+    r.litOff = (size_t)(f0 + b0);
+    return r;
+}
+__device__ __forceinline__ void put_hdr3(uint8_t* out, uint32_t h) { out[0] = (uint8_t)h; out[1] = (uint8_t)(h >> 8); out[2] = (uint8_t)(h >> 16); }
+
+// the compressed block if it is smaller than the input, else a raw block; returns the slot bytes
+__device__ uint32_t finish_block(uint8_t* out, const uint8_t* __restrict__ bsrc, uint32_t blkSize, uint32_t last, uint32_t bodySize, bool overCap, uint32_t lane) {
+    if (!overCap && bodySize < blkSize) {
+        if (lane == 0) put_hdr3(out, last | (2u << 1) | (bodySize << 3));
+        return 3 + bodySize;
+    }
+    __syncwarp();
+    if (lane == 0) put_hdr3(out, last | (blkSize << 3));
+    warp_copy(out + 3, bsrc, blkSize, lane);
+    return 3 + blkSize;
+}
+
+// ---------------------------------------------------------------- E1: tables and literals, one warp per block
 __global__ void __launch_bounds__(B2Z_ENT_WARPS * 32)
-zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
-                        const uint64_t* __restrict__ seqs, const uint32_t* __restrict__ nseqArr,
-                        const uint8_t* __restrict__ lits, const uint32_t* __restrict__ nlitArr,
-                        uint8_t* __restrict__ slots, uint32_t* __restrict__ slotSize, uint32_t nBlocks) {
+zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
+                       const uint64_t* __restrict__ seqs, const uint32_t* __restrict__ nseqArr,
+                       const uint8_t* __restrict__ lits, const uint32_t* __restrict__ nlitArr,
+                       uint8_t* __restrict__ slots, uint32_t* __restrict__ slotSize, uint8_t* __restrict__ scratch, uint32_t nBlocks) {
     __shared__ WarpWS wsAll[B2Z_ENT_WARPS];
     const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
     WarpWS* ws = &wsAll[wib];
-    const uint32_t blocksPerFrame = 1u << (g.frameLog - 17u);
     for (uint32_t blk = blockIdx.x * B2Z_ENT_WARPS + wib; blk < nBlocks; blk += gridDim.x * B2Z_ENT_WARPS) {
-        // geometry of this block
-        const uint64_t frame = blk / blocksPerFrame; const uint32_t bif = blk % blocksPerFrame;
-        const uint64_t f0 = frame << g.frameLog;
-        const uint64_t fn = enc_frame_bytes(g, srcSize, frame);
-        const uint64_t b0 = (uint64_t)bif << 17;
-        const uint32_t blkSize = (uint32_t)((fn - b0) < B2Z_BLOCK ? (fn - b0) : B2Z_BLOCK);
-        const uint32_t last = (b0 + blkSize == fn) ? 1u : 0u;
-        const uint8_t* bsrc = src + f0 + b0;
-        const uint8_t* lit = lits + f0 + b0;
+        const BlockGeom bg = block_geom(g, srcSize, blk);
+        const uint32_t blkSize = bg.blkSize, last = bg.last;
+        const uint8_t* bsrc = src + bg.litOff;
+        const uint8_t* lit = lits + bg.litOff;
         const uint64_t* sq = seqs + (size_t)blk * B2Z_MAXSEQ;
         const uint32_t nbSeq = nseqArr[blk], nlit = nlitArr[blk];
         uint8_t* out = slots + (size_t)blk * B2Z_SLOT;
         uint8_t* body = out + 3;
-        uint32_t outSize;
+        EntRec* rec = reinterpret_cast<EntRec*>(scratch + (size_t)blk * ENT_SCRATCH_STRIDE);
 
         // RLE block?
         bool rle = false;
@@ -418,7 +574,7 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
             rle = B2Z_SEQ_LL(s0) == 1 && B2Z_SEQ_ML(s0) == blkSize - 1u && B2Z_SEQ_OFFBASE(s0) == 4u;
         }
         if (rle) {
-            if (lane == 0) { const uint32_t h = last | (1u << 1) | (blkSize << 3); out[0] = (uint8_t)h; out[1] = (uint8_t)(h >> 8); out[2] = (uint8_t)(h >> 16); out[3] = bsrc[0]; slotSize[blk] = 4; }
+            if (lane == 0) { put_hdr3(out, last | (1u << 1) | (blkSize << 3)); out[3] = bsrc[0]; slotSize[blk] = 4; rec->run = 0; }
             continue;
         }
 
@@ -436,7 +592,7 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
         __syncwarp();
         uint32_t ns = 0;
         for (uint32_t i = lane; i < 256; i += 32) ns += ws->hist[i] != 0;
-        for (int d = 16; d; d >>= 1) ns += __shfl_xor_sync(B2Z_FULL, ns, d);
+        ns = warp_sum(ns);
 
         const uint32_t rawHdr = nlit < 32 ? 1u : (nlit < 4096 ? 2u : 3u);
         uint32_t litSecSize = 0;
@@ -445,7 +601,7 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
             if (lane == 0) {
                 if (rawHdr == 1) body[0] = (uint8_t)(1u | (nlit << 3));
                 else if (rawHdr == 2) { const uint32_t h = 1u | (1u << 2) | (nlit << 4); body[0] = (uint8_t)h; body[1] = (uint8_t)(h >> 8); }
-                else { const uint32_t h = 1u | (3u << 2) | (nlit << 4); body[0] = (uint8_t)h; body[1] = (uint8_t)(h >> 8); body[2] = (uint8_t)(h >> 16); }
+                else put_hdr3(body, 1u | (3u << 2) | (nlit << 4));
                 body[rawHdr] = lit[0];
             }
             litSecSize = rawHdr + 1; litDone = true;
@@ -453,17 +609,13 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
         if (!litDone && nlit >= B2Z_LIT_HUF_MIN && ns >= 2) {
             const bool four = nlit >= 256;
             const uint32_t lh = nlit < 1024 ? 3u : (nlit < 16384 ? 4u : 5u);
-            uint32_t ts = 0;
-            if (lane == 0) {
-                uint32_t maxSym; const uint32_t maxBits = huf_build(ws, &maxSym);
-                ts = huf_write_table(ws, body + lh, maxBits, maxSym);
-            }
-            ts = __shfl_sync(B2Z_FULL, ts, 0);
+            uint32_t maxSym; const uint32_t maxBits = huf_build(ws, lane, &maxSym);
+            const uint32_t ts = huf_write_table(ws, body + lh, maxBits, maxSym, lane);
             __syncwarp();
             // exact payload bits from the (unmodified) histogram; decide on the byte bound before writing
             uint32_t T = 0;
             for (uint32_t i = lane; i < 256; i += 32) T += ws->hist[i] * ws->hufLen[i];
-            for (int d = 16; d; d >>= 1) T += __shfl_xor_sync(B2Z_FULL, T, d);
+            T = warp_sum(T);
             const uint32_t est = ts + (four ? 6u : 0u) + ((T + 7u) >> 3) + (four ? 4u : 1u);
             if (ts && lh + est < rawHdr + nlit) {
                 uint8_t* p = body + lh + ts;
@@ -483,7 +635,7 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
                 const uint32_t csize = ts + bodySz;
                 if (lane == 0) {
                     const uint32_t sf = !four ? 0u : (lh == 3 ? 1u : (lh == 4 ? 2u : 3u));
-                    if (lh == 3) { const uint32_t h = 2u | (sf << 2) | (nlit << 4) | (csize << 14); body[0] = (uint8_t)h; body[1] = (uint8_t)(h >> 8); body[2] = (uint8_t)(h >> 16); }
+                    if (lh == 3) put_hdr3(body, 2u | (sf << 2) | (nlit << 4) | (csize << 14));
                     else if (lh == 4) { const uint32_t h = 2u | (sf << 2) | (nlit << 4) | (csize << 18); body[0] = (uint8_t)h; body[1] = (uint8_t)(h >> 8); body[2] = (uint8_t)(h >> 16); body[3] = (uint8_t)(h >> 24); }
                     else { const uint64_t h = 2ull | (sf << 2) | ((uint64_t)nlit << 4) | ((uint64_t)csize << 22);
                            body[0] = (uint8_t)h; body[1] = (uint8_t)(h >> 8); body[2] = (uint8_t)(h >> 16); body[3] = (uint8_t)(h >> 24); body[4] = (uint8_t)(h >> 32); }
@@ -495,14 +647,14 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
             if (lane == 0) {
                 if (rawHdr == 1) body[0] = (uint8_t)(nlit << 3);
                 else if (rawHdr == 2) { const uint32_t h = (1u << 2) | (nlit << 4); body[0] = (uint8_t)h; body[1] = (uint8_t)(h >> 8); }
-                else { const uint32_t h = (3u << 2) | (nlit << 4); body[0] = (uint8_t)h; body[1] = (uint8_t)(h >> 8); body[2] = (uint8_t)(h >> 16); }
+                else put_hdr3(body, (3u << 2) | (nlit << 4));
             }
             warp_copy(body + rawHdr, lit, nlit, lane);
             litSecSize = rawHdr + nlit;
         }
         __syncwarp();
 
-        // =========================== sequences section
+        // =========================== sequences section: header and tables
         uint8_t* sp = body + litSecSize;
         uint32_t seqSecSize;
         bool overCap = false;
@@ -518,107 +670,181 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
             for (uint32_t i = lane; i < 192; i += 32) ws->hist[i] = 0;
             __syncwarp();
             uint32_t extra = 0;                                   // sum of raw extra bits (for the size bound)
-            for (uint32_t i = lane; i < nbSeq; i += 32) {
-                const uint64_t s = sq[i];
-                const uint32_t cl = ll_code(B2Z_SEQ_LL(s)), cm = ml_code(B2Z_SEQ_ML(s) - 3u), co = highbit32(B2Z_SEQ_OFFBASE(s));
-                atomicAdd(&cLL[cl], 1u); atomicAdd(&cML[cm], 1u); atomicAdd(&cOF[co], 1u);
-                extra += d_LL_bits[cl] + d_ML_bits[cm] + co;
+            for (uint32_t i0 = 0; i0 < nbSeq; i0 += 128) {        // four records per lane in flight
+                uint64_t v[4];
+#pragma unroll
+                for (uint32_t m = 0; m < 4; m++) { const uint32_t i = i0 + 32u * m + lane; v[m] = i < nbSeq ? sq[i] : 0ull; }
+#pragma unroll
+                for (uint32_t m = 0; m < 4; m++) {
+                    const uint64_t s = v[m];
+                    if (!s) continue;                             // past the end (a record is never 0)
+                    const uint32_t cl = ll_code(B2Z_SEQ_LL(s)), cm = ml_code(B2Z_SEQ_ML(s) - 3u), co = highbit32(B2Z_SEQ_OFFBASE(s));
+                    atomicAdd(&cLL[cl], 1u); atomicAdd(&cML[cm], 1u); atomicAdd(&cOF[co], 1u);
+                    extra += d_LL_bits[cl] + d_ML_bits[cm] + co;
+                }
             }
-            for (int d = 16; d; d >>= 1) extra += __shfl_xor_sync(B2Z_FULL, extra, d);
+            extra = warp_sum(extra);
             __syncwarp();
             FseCT* ctL = &ws->u.fse.ct[0]; FseCT* ctO = &ws->u.fse.ct[1]; FseCT* ctM = &ws->u.fse.ct[2];
-            uint32_t tblBytes = 0;
-            if (lane == 0) {
-                uint8_t* tp = sp + seqSecSize + 1;
-                uint32_t mL, mO, mM;
-                tp += choose_seq_table(ws, ctL, tp, cLL, nbSeq, 35, 9, d_LL_defNorm, 35, 6, &mL);
-                tp += choose_seq_table(ws, ctO, tp, cOF, nbSeq, 31, 8, d_OF_defNorm, 28, 5, &mO);
-                tp += choose_seq_table(ws, ctM, tp, cML, nbSeq, 52, 9, d_ML_defNorm, 52, 6, &mM);
-                sp[seqSecSize] = (uint8_t)((mL << 6) | (mO << 4) | (mM << 2));
-                tblBytes = (uint32_t)(tp - (sp + seqSecSize + 1));
-            }
-            tblBytes = __shfl_sync(B2Z_FULL, tblBytes, 0);
-            __syncwarp();
-            seqSecSize += 1 + tblBytes;
-            {
-                const uint64_t upper = (uint64_t)nbSeq * (ctL->log + ctO->log + ctM->log) + 1ull + extra;
-                overCap = (uint64_t)litSecSize + seqSecSize + ((upper + 7ull) >> 3) > B2Z_BODY_CAP;
-            }
-            if (!overCap) {
-            // ---- bitstream: sequences walked last -> first, 32 per batch
-            Stager st; st.init(ws->stage, sp + seqSecSize, lane);
-            uint8_t* bsStart = st.out;
-            uint32_t stL = 0, stO = 0, stM = 0;                   // chain states: valid on lanes 0,1,2
-            bool first = true;
-            for (uint32_t hi = nbSeq; hi > 0;) {
-                const uint32_t cnt = hi < 32u ? hi : 32u;
-                uint32_t llv = 0, mlv = 0, obv = 1, cl = 0, cm = 0, co = 0;
-                if (lane < cnt) {
-                    const uint64_t s = sq[hi - 1u - lane];
-                    llv = B2Z_SEQ_LL(s); mlv = B2Z_SEQ_ML(s); obv = B2Z_SEQ_OFFBASE(s);
-                    cl = ll_code(llv); cm = ml_code(mlv - 3u); co = highbit32(obv);
-                    ws->bcode[0][lane] = (uint8_t)cl; ws->bcode[1][lane] = (uint8_t)co; ws->bcode[2][lane] = (uint8_t)cm;
+            uint8_t* tp = sp + seqSecSize + 1;
+            uint32_t mL, mO, mM;
+            tp += choose_seq_table(ws, ctL, tp, cLL, nbSeq, 35, 9, d_LL_defNorm, 35, 6, &mL, lane);
+            tp += choose_seq_table(ws, ctO, tp, cOF, nbSeq, 31, 8, d_OF_defNorm, 28, 5, &mO, lane);
+            tp += choose_seq_table(ws, ctM, tp, cML, nbSeq, 52, 9, d_ML_defNorm, 52, 6, &mM, lane);
+            if (lane == 0) sp[seqSecSize] = (uint8_t)((mL << 6) | (mO << 4) | (mM << 2));
+            seqSecSize += 1 + (uint32_t)(tp - (sp + seqSecSize + 1));
+            const uint64_t upper = (uint64_t)nbSeq * (ctL->log + ctO->log + ctM->log) + 1ull + extra;
+            overCap = (uint64_t)litSecSize + seqSecSize + ((upper + 7ull) >> 3) > B2Z_BODY_CAP;
+            if (!overCap) {                                       // hand the tables to E2 and the sizes to E3
+                for (uint32_t i = lane; i < ENT_ST_N; i += 32)
+                    rec->tab.state[i] = i < ENT_ST_OF ? ctL->state[i] : (i < ENT_ST_ML ? ctO->state[i - ENT_ST_OF] : ctM->state[i - ENT_ST_ML]);
+                for (uint32_t i = lane; i < ENT_SY_N; i += 32) {
+                    const FseCT* ct = i < ENT_SY_OF ? ctL : (i < ENT_SY_ML ? ctO : ctM);
+                    const uint32_t s = i < ENT_SY_OF ? i : (i < ENT_SY_ML ? i - ENT_SY_OF : i - ENT_SY_ML);
+                    rec->tab.sym[i] = make_uint2(ct->dnb[s], (uint32_t)ct->dfs[s]);
                 }
+                if (lane == 0) { rec->run = 1; rec->bodyHead = litSecSize + seqSecSize; rec->logs = ctL->log | (ctO->log << 8) | (ctM->log << 16); }
                 __syncwarp();
-                if (lane < 3) {                                   // the three FSE chains
-                    const FseCT* ct = lane == 0 ? ctL : (lane == 1 ? ctO : ctM);
-                    uint32_t state = lane == 0 ? stL : (lane == 1 ? stO : stM);
-                    uint32_t k = 0;
-                    if (first) { state = fse_init_state(ct, ws->bcode[lane][0]); ws->bbits[lane][0] = 0; ws->bnb[lane][0] = 0; k = 1; }
-                    for (; k < cnt; k++) {
-                        uint32_t nb; const uint32_t bits = fse_encode(ct, &state, ws->bcode[lane][k], &nb);
-                        ws->bbits[lane][k] = (uint16_t)bits; ws->bnb[lane][k] = (uint8_t)nb;
-                    }
-                    if (lane == 0) stL = state; else if (lane == 1) stO = state; else stM = state;
-                }
-                __syncwarp();
-                // assemble: OF state, ML state, LL state, then LL, ML, OF extra bits
-                uint64_t lo = 0; uint32_t hiw = 0, nb = 0;
-                if (lane < cnt) {
-                    const uint32_t nO = ws->bnb[1][lane], nM = ws->bnb[2][lane], nL = ws->bnb[0][lane];
-                    lo = ws->bbits[1][lane]; nb = nO;
-                    lo |= (uint64_t)ws->bbits[2][lane] << nb; nb += nM;
-                    lo |= (uint64_t)ws->bbits[0][lane] << nb; nb += nL;                  // <= 26 bits
-                    const uint32_t lb = d_LL_bits[cl], mb = d_ML_bits[cm];
-                    lo |= (uint64_t)(llv - d_LL_base[cl]) << nb; nb += lb;                 // <= 42
-                    lo |= (uint64_t)(mlv - d_ML_base[cm]) << nb; nb += mb;                 // <= 58
-                    const uint32_t ox = obv - (1u << co);
-                    if (nb + co <= 64) { lo |= (co ? ((uint64_t)ox << nb) : 0ull); }
-                    else { lo |= (uint64_t)ox << nb; hiw = (uint32_t)((uint64_t)ox >> (64u - nb)); }
-                    nb += co;
-                }
-                uint32_t total; const uint32_t off = warp_excl_scan(nb, lane, &total);
-                st.put(st.bits + off, lo, hiw, nb);
-                st.bits += total; hi -= cnt; first = false;
-                if (st.bits > STAGE_FLUSH_BITS) st.flush(lane, false);
-            }
-            // final states: ML, OF, LL, then end mark
-            {
-                const uint32_t sM = __shfl_sync(B2Z_FULL, stM, 2), sO = __shfl_sync(B2Z_FULL, stO, 1), sL = __shfl_sync(B2Z_FULL, stL, 0);
-                if (lane == 0) {
-                    uint32_t o = st.bits;
-                    st.put(o, sM & ((1u << ctM->log) - 1u), 0, ctM->log); o += ctM->log;
-                    st.put(o, sO & ((1u << ctO->log) - 1u), 0, ctO->log); o += ctO->log;
-                    st.put(o, sL & ((1u << ctL->log) - 1u), 0, ctL->log); o += ctL->log;
-                    st.put(o, 1, 0, 1);
-                }
-                st.bits += ctM->log + ctO->log + ctL->log + 1u;
-                st.flush(lane, true);
-            }
-            seqSecSize += (uint32_t)(st.out - bsStart);
+                continue;
             }
         }
         __syncwarp();
-        const uint32_t bodySize = litSecSize + seqSecSize;
-        if (!overCap && bodySize < blkSize) {
-            if (lane == 0) { const uint32_t h = last | (2u << 1) | (bodySize << 3); out[0] = (uint8_t)h; out[1] = (uint8_t)(h >> 8); out[2] = (uint8_t)(h >> 16); }
-            outSize = 3 + bodySize;
-        } else {
-            if (lane == 0) { const uint32_t h = last | (blkSize << 3); out[0] = (uint8_t)h; out[1] = (uint8_t)(h >> 8); out[2] = (uint8_t)(h >> 16); }
-            __syncwarp();
-            warp_copy(out + 3, bsrc, blkSize, lane);
-            outSize = 3 + blkSize;
+        const uint32_t outSize = finish_block(out, bsrc, blkSize, last, litSecSize + seqSecSize, overCap, lane);
+        if (lane == 0) { slotSize[blk] = outSize; rec->run = 0; }
+        __syncwarp();
+    }
+}
+
+// ---------------------------------------------------------------- E2: the FSE state chains, 30 per warp
+// The sequence records are read a chunk at a time by the whole warp (ENT_CHAIN_SEQS per block, all loads in flight together)
+// and reduced to their three codes in shared memory, so the chains themselves wait on shared memory only.
+#define ENT_CHAIN_BLOCKS 10
+#define ENT_CHAIN_SEQS   48
+#define ENT_CHAIN_LOADS  (ENT_CHAIN_BLOCKS * ENT_CHAIN_SEQS / 32)
+__global__ void __launch_bounds__(32)
+zstd_enc_chains_kernel(const uint64_t* __restrict__ seqs, const uint32_t* __restrict__ nseqArr, uint8_t* __restrict__ scratch, uint32_t nBlocks) {
+    __shared__ EntTables tabs[ENT_CHAIN_BLOCKS];
+    __shared__ uint32_t codes[ENT_CHAIN_BLOCKS][ENT_CHAIN_SEQS];   // LL | OF << 8 | ML << 16 of walk steps k0 .. k0 + 47
+    __shared__ uint32_t nsq[ENT_CHAIN_BLOCKS];
+    const uint32_t lane = threadIdx.x, b = lane / 3u, t = lane - 3u * b;
+    for (uint32_t blk0 = blockIdx.x * ENT_CHAIN_BLOCKS; blk0 < nBlocks; blk0 += gridDim.x * ENT_CHAIN_BLOCKS) {
+        const uint32_t nb = nBlocks - blk0 < ENT_CHAIN_BLOCKS ? nBlocks - blk0 : ENT_CHAIN_BLOCKS;
+        // stage the group's tables (whole EntTables, 16 bytes per lane per step)
+        for (uint32_t j = 0; j < nb; j++) {
+            const EntRec* r = reinterpret_cast<const EntRec*>(scratch + (size_t)(blk0 + j) * ENT_SCRATCH_STRIDE);
+            if (!r->run) continue;
+            const uint4* s4 = reinterpret_cast<const uint4*>(&r->tab);
+            uint4* d4 = reinterpret_cast<uint4*>(&tabs[j]);
+            for (uint32_t i = lane; i < sizeof(EntTables) / 16u; i += 32) d4[i] = s4[i];
         }
+        if (lane < ENT_CHAIN_BLOCKS)
+            nsq[lane] = lane < nb && reinterpret_cast<const EntRec*>(scratch + (size_t)(blk0 + lane) * ENT_SCRATCH_STRIDE)->run ? nseqArr[blk0 + lane] : 0u;
+        __syncwarp();
+        const uint32_t blk = blk0 + b;
+        const bool mine = b < nb;
+        const uint32_t n = mine ? nsq[b] : 0u;
+        EntRec* rec = reinterpret_cast<EntRec*>(scratch + (size_t)(mine ? blk : blk0) * ENT_SCRATCH_STRIDE);
+        uint32_t* words = reinterpret_cast<uint32_t*>(scratch + (size_t)blk * ENT_SCRATCH_STRIDE + sizeof(EntRec));
+        const uint16_t* stT = tabs[mine ? b : 0].state + (t == 0 ? 0u : (t == 1 ? ENT_ST_OF : ENT_ST_ML));
+        const uint2* syT = tabs[mine ? b : 0].sym + (t == 0 ? 0u : (t == 1 ? ENT_SY_OF : ENT_SY_ML));
+        const uint32_t nMax = warp_max(n);
+        uint32_t state = 0;
+        for (uint32_t k0 = 0; k0 < nMax; k0 += ENT_CHAIN_SEQS) {
+            // codes of walk steps k0 .. k0 + 47 of every block (sequence n - 1 - k)
+            uint64_t v[ENT_CHAIN_LOADS];
+#pragma unroll
+            for (uint32_t m = 0; m < ENT_CHAIN_LOADS; m++) {
+                const uint32_t j = lane + 32u * m, bj = j / ENT_CHAIN_SEQS, k = k0 + j % ENT_CHAIN_SEQS, nj = nsq[bj];
+                v[m] = k < nj ? seqs[(size_t)(blk0 + bj) * B2Z_MAXSEQ + (nj - 1u - k)] : 0ull;
+            }
+#pragma unroll
+            for (uint32_t m = 0; m < ENT_CHAIN_LOADS; m++) {
+                const uint32_t j = lane + 32u * m;
+                const uint64_t s = v[m];
+                codes[j / ENT_CHAIN_SEQS][j % ENT_CHAIN_SEQS] = s ? ll_code(B2Z_SEQ_LL(s)) | (highbit32(B2Z_SEQ_OFFBASE(s)) << 8) | (ml_code(B2Z_SEQ_ML(s) - 3u) << 16) : 0u;
+            }
+            __syncwarp();
+            const uint32_t kEnd = nMax - k0 < ENT_CHAIN_SEQS ? nMax - k0 : ENT_CHAIN_SEQS;
+            for (uint32_t kk = 0; kk < kEnd; kk++) {
+                const uint32_t k = k0 + kk;
+                const bool act = k < n;
+                uint32_t bits = 0, nbits = 0;
+                if (act) {
+                    const uint32_t sym = (codes[b][kk] >> (8u * t)) & 255u;
+                    const uint2 e = syT[sym];
+                    if (k == 0) {                                   // the last sequence sets the initial state
+                        const uint32_t nb0 = (e.x + (1u << 15)) >> 16;
+                        state = stT[(((nb0 << 16) - e.x) >> nb0) + e.y];
+                    } else {
+                        nbits = (state + e.x) >> 16; bits = state & ((1u << nbits) - 1u);
+                        state = stT[(state >> nbits) + e.y];
+                    }
+                }
+                // lane 3b gathers OF (3b+1) and ML (3b+2) and writes OF | ML | LL with the bit count on top
+                const uint32_t oB = __shfl_down_sync(B2Z_FULL, bits, 1), oN = __shfl_down_sync(B2Z_FULL, nbits, 1);
+                const uint32_t mB = __shfl_down_sync(B2Z_FULL, bits, 2), mN = __shfl_down_sync(B2Z_FULL, nbits, 2);
+                if (act && t == 0) words[n - 1u - k] = oB | (mB << oN) | (bits << (oN + mN)) | ((oN + mN + nbits) << 26);
+            }
+            __syncwarp();
+        }
+        if (n) rec->fin[t] = (uint16_t)state;
+        __syncwarp();
+    }
+}
+
+// ---------------------------------------------------------------- E3: the sequence bitstream, one warp per block
+__global__ void __launch_bounds__(B2Z_ENT_WARPS * 32)
+zstd_enc_seqbits_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
+                        const uint64_t* __restrict__ seqs, const uint32_t* __restrict__ nseqArr,
+                        uint8_t* __restrict__ slots, uint32_t* __restrict__ slotSize, const uint8_t* __restrict__ scratch, uint32_t nBlocks) {
+    __shared__ uint32_t stageAll[B2Z_ENT_WARPS][STAGE_WORDS];
+    const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
+    for (uint32_t blk = blockIdx.x * B2Z_ENT_WARPS + wib; blk < nBlocks; blk += gridDim.x * B2Z_ENT_WARPS) {
+        const EntRec* rec = reinterpret_cast<const EntRec*>(scratch + (size_t)blk * ENT_SCRATCH_STRIDE);
+        if (!rec->run) continue;
+        const uint32_t* words = reinterpret_cast<const uint32_t*>(scratch + (size_t)blk * ENT_SCRATCH_STRIDE + sizeof(EntRec));
+        const BlockGeom bg = block_geom(g, srcSize, blk);
+        const uint64_t* sq = seqs + (size_t)blk * B2Z_MAXSEQ;
+        const uint32_t nbSeq = nseqArr[blk], bodyHead = rec->bodyHead, logs = rec->logs;
+        const uint32_t logL = logs & 255u, logO = (logs >> 8) & 255u, logM = logs >> 16;
+        uint8_t* out = slots + (size_t)blk * B2Z_SLOT;
+        Stager st; st.init(stageAll[wib], out + 3 + bodyHead, lane);
+        uint8_t* bsStart = st.out;
+        // sequences walked last -> first, 32 per step: state bits (OF, ML, LL), then LL, ML, OF extra bits
+        for (uint32_t hi = nbSeq; hi > 0;) {
+            const uint32_t cnt = hi < 32u ? hi : 32u;
+            uint64_t lo = 0; uint32_t hiw = 0, nb = 0;
+            if (lane < cnt) {
+                const uint32_t i = hi - 1u - lane;
+                const uint64_t s = sq[i]; const uint32_t w = words[i];
+                const uint32_t llv = B2Z_SEQ_LL(s), mlv = B2Z_SEQ_ML(s), obv = B2Z_SEQ_OFFBASE(s);
+                const uint32_t cl = ll_code(llv), cm = ml_code(mlv - 3u), co = highbit32(obv);
+                lo = w & 0x3FFFFFFu; nb = w >> 26;                                     // <= 26 bits
+                const uint32_t lb = d_LL_bits[cl], mb = d_ML_bits[cm];
+                lo |= (uint64_t)(llv - d_LL_base[cl]) << nb; nb += lb;                 // <= 42
+                lo |= (uint64_t)(mlv - d_ML_base[cm]) << nb; nb += mb;                 // <= 58
+                const uint32_t ox = obv - (1u << co);
+                if (nb + co <= 64) { lo |= (co ? ((uint64_t)ox << nb) : 0ull); }
+                else { lo |= (uint64_t)ox << nb; hiw = (uint32_t)((uint64_t)ox >> (64u - nb)); }
+                nb += co;
+            }
+            uint32_t total; const uint32_t off = warp_excl_scan(nb, lane, &total);
+            st.put(st.bits + off, lo, hiw, nb);
+            st.bits += total; hi -= cnt;
+            if (st.bits > STAGE_FLUSH_BITS) st.flush(lane, false);
+        }
+        // final states: ML, OF, LL, then end mark
+        if (lane == 0) {
+            uint32_t o = st.bits;
+            st.put(o, rec->fin[2] & ((1u << logM) - 1u), 0, logM); o += logM;
+            st.put(o, rec->fin[1] & ((1u << logO) - 1u), 0, logO); o += logO;
+            st.put(o, rec->fin[0] & ((1u << logL) - 1u), 0, logL); o += logL;
+            st.put(o, 1, 0, 1);
+        }
+        st.bits += logM + logO + logL + 1u;
+        st.flush(lane, true);
+        const uint32_t bodySize = bodyHead + (uint32_t)(st.out - bsStart);
+        const uint32_t outSize = finish_block(out, src + bg.litOff, bg.blkSize, bg.last, bodySize, false, lane);
         if (lane == 0) slotSize[blk] = outSize;
         __syncwarp();
     }
@@ -627,12 +853,32 @@ zstd_enc_entropy_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
 #ifndef B2Z_CUEMU
 void launch_zstd_enc_entropy(const uint8_t* src, uint64_t srcSize, const EncGeom& g,
                              const uint64_t* seqs, const uint32_t* nseq, const uint8_t* lits, const uint32_t* nlit,
-                             uint8_t* slots, uint32_t* slotSize, uint32_t nBlocks, uint32_t smCount, cudaStream_t st) {
+                             uint8_t* slots, uint32_t* slotSize, uint8_t* scratch, uint32_t nBlocks, uint32_t smCount, cudaStream_t st) {
     if (!nBlocks) return;
     uint32_t grid = (nBlocks + B2Z_ENT_WARPS - 1) / B2Z_ENT_WARPS;
     const uint32_t cap = smCount * 16u;
     if (grid > cap) grid = cap;
-    zstd_enc_entropy_kernel<<<grid, B2Z_ENT_WARPS * 32, 0, st>>>(src, srcSize, g, seqs, nseq, lits, nlit, slots, slotSize, nBlocks);
+    zstd_enc_tables_kernel<<<grid, B2Z_ENT_WARPS * 32, 0, st>>>(src, srcSize, g, seqs, nseq, lits, nlit, slots, slotSize, scratch, nBlocks);
+    zstd_enc_chains_kernel<<<(nBlocks + ENT_CHAIN_BLOCKS - 1) / ENT_CHAIN_BLOCKS, 32, 0, st>>>(seqs, nseq, scratch, nBlocks);
+    zstd_enc_seqbits_kernel<<<grid, B2Z_ENT_WARPS * 32, 0, st>>>(src, srcSize, g, seqs, nseq, slots, slotSize, scratch, nBlocks);
+}
+#else
+// Host emulation (tests/cuemu): the emulator's stage E entry launches zstd_enc_entropy_kernel once, over 4-warp CTAs of the
+// blocks.  Stage E is three launches with scratch between them, so under the emulator that entry's first thread runs E1, E2
+// and E3 in turn over every block -- the launches launch_zstd_enc_entropy makes -- with scratch of its own, and counts their
+// collectives as its own.  Every other thread returns at once.
+inline void zstd_enc_entropy_kernel(const uint8_t* src, uint64_t srcSize, EncGeom g, const uint64_t* seqs, const uint32_t* nseq,
+                                    const uint8_t* lits, const uint32_t* nlit, uint8_t* slots, uint32_t* slotSize, uint32_t nBlocks) {
+    if (blockIdx.x != 0 || threadIdx.x != 0 || !nBlocks) return;
+    cuemu::Block* const outer = cuemu::blk();
+    std::vector<uint8_t> buf((size_t)nBlocks * ENT_SCRATCH_STRIDE + 16, 0xCD);
+    uint8_t* const scratch = buf.data() + ((16u - ((uintptr_t)buf.data() & 15u)) & 15u);
+    const dim3 grid((nBlocks + B2Z_ENT_WARPS - 1) / B2Z_ENT_WARPS), block(B2Z_ENT_WARPS * 32);
+    uint64_t c = cuemu::launch(grid, block, 0, [&] { zstd_enc_tables_kernel(src, srcSize, g, seqs, nseq, lits, nlit, slots, slotSize, scratch, nBlocks); });
+    c += cuemu::launch(dim3((nBlocks + ENT_CHAIN_BLOCKS - 1) / ENT_CHAIN_BLOCKS), dim3(32), 0, [&] { zstd_enc_chains_kernel(seqs, nseq, scratch, nBlocks); });
+    c += cuemu::launch(grid, block, 0, [&] { zstd_enc_seqbits_kernel(src, srcSize, g, seqs, nseq, slots, slotSize, scratch, nBlocks); });
+    cuemu::blk() = outer;                                        // each launch leaves the emulator without a current CTA
+    outer->collectives += c;
 }
 #endif
 
