@@ -352,7 +352,8 @@ class Codec:
         return v.value
 
     def xz_compress(self, data, check=4, filter_id=0, filter_prop=0) -> bytes:
-        """-> .xz file bytes: one Block per frame; check 0 none, 1 CRC32, 4 CRC64; filter_id: 0 or a Codec.filter id run in front of LZMA2"""
+        """-> .xz file bytes: one Block per frame; check 0 none, 1 CRC32, 4 CRC64; filter_id: 0 or a Codec.filter id run in front of LZMA2,
+        every Block on its own (filter_prop: delta distance or start offset; RISC-V 0x0B writes xz filter 0x0B)"""
         import numpy as np
         src = np.frombuffer(data, dtype=np.uint8) if len(data) else np.zeros(1, dtype=np.uint8)
         cap = self.L.b200z_xz_compress_bound(self.h, len(data))
@@ -372,7 +373,8 @@ class Codec:
         return out[:sz.value].tobytes()
 
     def filter(self, method_id, encode, data, prop=0) -> bytes:
-        """Delta (0x03, prop = distance) / branch converters ARM64 0x0A, ARM 0x03030501, PPC 0x03030205, SPARC 0x03030805 (prop = start offset)"""
+        """Delta (0x03, prop = distance) / branch converters x86 0x03030103, ARM64 0x0A, ARM 0x03030501, ARM Thumb 0x03030701, PPC 0x03030205,
+        SPARC 0x03030805, RISC-V 0x0B (prop = start offset; even for RISC-V and Thumb, else B200zError -6).  BCJ2 and IA64: error -6"""
         import numpy as np
         buf = np.frombuffer(bytearray(data), dtype=np.uint8) if len(data) else np.zeros(1, dtype=np.uint8)
         self._check(self.L.b200z_filter_host(self.h, method_id, 1 if encode else 0, buf.ctypes.data, len(data), prop))

@@ -17,6 +17,7 @@
 #define B200Z_F_ARM   0x03030501u
 #define B200Z_F_ARMT  0x03030701u
 #define B200Z_F_SPARC 0x03030805u
+#define B200Z_F_RISCV 0x0Bu
 
 B2Z_HD uint32_t b2z_bswap32(uint32_t v) { return (v >> 24) | ((v >> 8) & 0xFF00u) | ((v << 8) & 0xFF0000u) | (v << 24); }
 
@@ -85,6 +86,57 @@ B2Z_HD int b2z_x86_convert(uint32_t hist, uint32_t operand, uint32_t next, int e
     if (hist != 0u && b2z_x86_is_00_ff(v >> (8u * fix))) { v ^= (0x100u << (8u * fix)) - 1u; v = enc ? v + next : v - next; }
     *out = (v & 0x1FFFFFFu) - (1u << 24);
     return 1;
+}
+
+/* ---- RISC-V (C/Bra.c:426-709).  A scan over even positions p with p + 8 <= (n & ~1) whose step (2, 4, 6 or 8 bytes) depends on the
+ * instruction at p.  w0 / w1 = the little-endian words at p and p + 4, as they were BEFORE the scan wrote anything at or after p.
+ *   JAL with rd = x1 / x5 (a call): its 21-bit offset becomes absolute, bits 20:1 stored big-endian over bytes 1.5 .. 3; step 4.
+ *   AUIPC rd (rd not x0 / x2) followed by a 32-bit instruction whose rs1 = rd (auipc + jalr / load / addi): the pair's combined
+ *     offset becomes absolute and is stored big-endian in the second word; the first becomes "AUIPC x2" holding the second
+ *     instruction's low 20 bits; step 8.  Without such a partner: step 6 (the partner's slot is not looked at again as a start).
+ *   AUIPC x0 / x2: a real "AUIPC x2" that looks like a converted pair (bits 13:12 = 3, bits 31:27 not x0 / x2) is escaped by
+ *     swapping fields between its two words, so that decoding can tell the two apart; step 8.  Otherwise step 4.
+ *   anything else: step 2.
+ * The step is the same when encoding and when decoding (both read the same fields), and a conversion writes only inside
+ * [p, p + step) -- so the positions the scan visits are a pure function of the input bytes.  b2z_filter.cu builds on that. */
+/* -> the step at a position; bit 0 set = the position converts (JAL: w0 only; AUIPC: w0 and w1) */
+B2Z_HD uint32_t b2z_riscv_scan(uint32_t w0, uint32_t w1) {
+    const uint32_t op = w0 & 0x7Fu, rd = (w0 >> 7) & 0x1Fu;
+    if (op == 0x6Fu) return (rd == 1u || rd == 5u) ? 5u : 2u;
+    if (op != 0x17u) return 2u;
+    if (rd != 0u && rd != 2u) return ((w1 & 3u) == 3u && ((w1 >> 15) & 0x1Fu) == rd) ? 9u : 6u;
+    return (rd == 2u && ((w0 >> 12) & 3u) == 3u && ((w0 >> 27) & 0x1Du) != 0u) ? 9u : 4u;
+}
+B2Z_HD uint32_t b2z_riscv_jal_offset(uint32_t w) {                  /* the J-immediate, bits 20:1 (unsigned) */
+    return ((w >> 11) & 0x100000u) | ((w >> 20) & 0x7FEu) | ((w >> 9) & 0x800u) | (w & 0xFF000u);
+}
+/* a converting position (b2z_riscv_scan bit 0) at address ia: rewrites *w0 (and *w1 for the 8-byte forms) */
+B2Z_HD void b2z_riscv_enc(uint32_t *w0, uint32_t *w1, uint32_t ia) {
+    const uint32_t a = *w0, b = *w1;
+    if ((a & 0x7Fu) == 0x6Fu) {
+        const uint32_t t = b2z_riscv_jal_offset(a) + ia;
+        *w0 = (a & 0xFFFu) | (((t >> 17) & 0xFu) << 12) | (((t >> 9) & 0xFFu) << 16) | (((t >> 1) & 0xFFu) << 24);
+    } else if (((a >> 7) & 0x1Fu) != 2u) {                          /* auipc rd + partner -> "auipc x2 | partner" + absolute target */
+        *w0 = (b << 12) | (2u << 7) | 0x17u;
+        *w1 = b2z_bswap32((a & 0xFFFFF000u) + (uint32_t)((int32_t)b >> 20) + ia);
+    } else {                                                        /* escape a real auipc x2 */
+        *w0 = ((a >> 27) << 7) | 0x17u | (b & 0xFFFFF000u);
+        *w1 = (a >> 12) | (b << 20);
+    }
+}
+B2Z_HD void b2z_riscv_dec(uint32_t *w0, uint32_t *w1, uint32_t ia) {
+    const uint32_t a = *w0, b = *w1;
+    if ((a & 0x7Fu) == 0x6Fu) {
+        const uint32_t off = ((((a >> 12) & 0xFu) << 17) | (((a >> 16) & 0xFFu) << 9) | (((a >> 24) & 0xFFu) << 1)) - ia;
+        *w0 = (a & 0xFFFu) | ((off & 0x100000u) << 11) | ((off & 0x7FEu) << 20) | ((off & 0x800u) << 9) | (off & 0xFF000u);
+    } else if (((a >> 7) & 0x1Fu) == 2u) {                          /* a converted pair: rebuild auipc rd + partner */
+        const uint32_t t = b2z_bswap32(b) - ia;
+        *w0 = ((a >> 27) << 7) | 0x17u | ((t + 0x800u) & 0xFFFFF000u);
+        *w1 = (a >> 12) | (t << 20);
+    } else {                                                        /* an escaped auipc x2 */
+        *w0 = (b << 12) | (2u << 7) | 0x17u;
+        *w1 = (a & 0xFFFFF000u) | (b >> 20);
+    }
 }
 
 #endif

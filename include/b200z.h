@@ -212,7 +212,7 @@ uint64_t b200z_crc64_combine(uint64_t crcA, uint64_t crcB, uint64_t lenB);
 /* ---- .xz container around the LZMA2 coder (SURVEY.md 8(f) item 2) ----------------------------------------------------------
  * Replaces NCompress::NXz::CEncoder / CDecoder (CPP/7zip/Compress/XzEncoder.cpp, XzDecoder.cpp) -> Xz_Encode (C/XzEnc.c:1236) /
  * XzDecMt_Decode (C/XzDec.c).  The reader takes Blocks whose filter chain is LZMA2, optionally behind Delta / x86 / PowerPC / ARM / ARM Thumb / SPARC /
- * ARM64 filters (undone on the GPU); the writer emits LZMA2, optionally behind one of those filters (applied on the GPU per Block).  The writer emits one Block per 2^FRAMELOG input
+ * ARM64 / RISC-V filters (undone on the GPU; IA64 is B200Z_E_UNSUPPORTED); the writer emits LZMA2, optionally behind one of those filters (applied on the GPU per Block).  The writer emits one Block per 2^FRAMELOG input
  * bytes with both sizes in the Block header (the layout multi-threaded xz coders write); check type 0 none, 1 CRC32, 4 CRC64
  * (XZ_CHECK_*, C/Xz.h:31-35).  b200z_xz_wrap / b200z_xz_parse are the host-side container logic alone (no device needed). */
 typedef struct {
@@ -233,8 +233,9 @@ int b200z_xz_decompress_host(b200z_ctx *ctx, const void *src, size_t srcSize, vo
 
 /* ---- pre/post filters of a 7z folder / xz filter chain on the GPU (SURVEY.md 8(f) item 3) -----------------------------------
  * In place.  methodId = 7-Zip's filter id: 0x03 Delta (prop = distance 1..256; CPP/7zip/Compress/DeltaFilter.cpp, C/Delta.c),
- * 0x03030103 x86 BCJ (C/Bra86.c), 0x0A ARM64, 0x03030501 ARM, 0x03030701 ARM Thumb, 0x03030205 PPC, 0x03030805 SPARC (prop = start offset;
- * BranchMisc.cpp -> C/Bra.c z7_BranchConv_*).  BCJ2, RISCV, IA64 return B200Z_E_UNSUPPORTED. */
+ * 0x03030103 x86 BCJ (C/Bra86.c), 0x0A ARM64, 0x03030501 ARM, 0x03030701 ARM Thumb, 0x03030205 PPC, 0x03030805 SPARC, 0x0B RISCV (prop = start offset,
+ * even for RISCV and ARM Thumb; BranchMisc.cpp -> C/Bra.c z7_BranchConv_*; an odd RISCV offset is B200Z_E_UNSUPPORTED; no alignment
+ * requirement on the RISCV buffer).  BCJ2 and IA64 return B200Z_E_UNSUPPORTED. */
 int b200z_filter_device(b200z_ctx *ctx, uint32_t methodId, int encode, void *d_data, size_t n, uint32_t prop);
 int b200z_filter_host(b200z_ctx *ctx, uint32_t methodId, int encode, void *data, size_t n, uint32_t prop);
 
