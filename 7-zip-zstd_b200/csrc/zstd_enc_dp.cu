@@ -6,13 +6,15 @@
 //      price = log2(total / count) in 1/16 bit, clamped;
 //   2. per lane, a backward dynamic programme over its segment: cost[i] = min(literal + cost[i+1], the position's
 //      candidate (stage F) at its length L, L-1, L-2: B2Z_DP_MATCH + offset extra bits + cost[i+l]).  Only the
-//      next B2Z_CAP costs are live (candidates are at most B2Z_CAP long), kept in a per-lane ring in shared memory; the choice
-//      (0 = literal, else the length) goes to a byte array in HBM, four positions per store;
+//      next B2Z_CAP costs are live (candidates are at most B2Z_CAP long), kept in a per-lane ring in shared memory, cost[i+1]
+//      also in a register, and the match price is formed four positions ahead of the chain (dp_match); the choice (0 = literal,
+//      else the length) goes to a byte array in HBM, four positions per store;
 //   3. per lane, a forward walk that only counts (sequences, literals, where the last match ends) -- a chosen match of
 //      the full B2Z_CAP bytes is extended by direct comparison to the segment end;
 //   4. warp scans turn the counts into each lane's place in the block's sequence and literal arrays and into the literal
 //      run that reaches into a lane from the lanes before it;
-//   5. the same walk again, emitting final (offBase, litLength, matchLength) records and the literal bytes.  The repcode
+//   5. the same walk again, emitting final (offBase, litLength, matchLength) records and the literal bytes (a tile's literals
+//      one lane's run per store, dp_emit_literals).  The repcode
 //      history is "unknown" at every segment start, so no lane waits for another.
 // A block of one repeated byte becomes the single sequence that stage E stores as an RLE block.
 //
@@ -39,6 +41,18 @@ struct DpWarpSmem {
     uint8_t litc[256];
 };
 
+// -DB2Z_DP_CLOCKS (off by default; tools/enc_parse_profile.py --build-clocks): every warp adds the clock64() cycles it spends in each
+// phase to dp_clocks[]; b200z_dp_clocks() reads and clears them.  Without the switch the ticks compile to nothing.
+enum { DPC_HIST, DPC_DP_LOAD, DPC_DP, DPC_DP_STORE, DPC_CNT_LOAD, DPC_CNT, DPC_SCAN, DPC_EMIT_LOAD, DPC_EMIT, DPC_N };
+#ifdef B2Z_DP_CLOCKS
+__device__ unsigned long long dp_clocks[DPC_N + 1];                         // [DPC_N] = warps
+#define DP_TICK(ph) do { const long long now_ = clock64(); dpc[ph] += (unsigned long long)(now_ - dpLast); dpLast = now_; } while (0)
+#define DP_CLOCKS_FLUSH() do { if (lane == 0) { for (int p_ = 0; p_ < DPC_N; p_++) atomicAdd(&dp_clocks[p_], dpc[p_]); atomicAdd(&dp_clocks[DPC_N], 1ull); } } while (0)
+#else
+#define DP_TICK(ph) do { } while (0)
+#define DP_CLOCKS_FLUSH() do { } while (0)
+#endif
+
 // 16 * log2(x) as b2z_zstd_cost.h:zop_log16, with the fraction table in registers
 __device__ __forceinline__ uint32_t dp_log16(uint32_t x) {
     const uint32_t hb = highbit32(x);
@@ -49,21 +63,34 @@ __device__ __forceinline__ uint32_t dp_log16(uint32_t x) {
     return 16u * hb + ((k == 0u && (x & (x - 1u)) == 0u) ? 0u : fr);
 }
 
-// tile t of a 32-bit-per-position array: 32 coalesced 128-byte rows.  base = the block's array, bn = positions in the block
-__device__ __forceinline__ void dp_load_cand_tile(DpWarpSmem& sm, const uint32_t* __restrict__ base, uint32_t bn, uint32_t t, uint32_t lane) {
-#pragma unroll 8
+// Tiles are fetched into registers one tile ahead of the pass that uses them (fetch t+1 -- or t-1 in the backward DP -- right after
+// putting tile t into shared memory), so a tile's loads are in flight while the warp works on the one before: r[j] = row j's word in
+// column `lane`.  40 (DP pass) to 48 (emit pass) registers per lane: 128 in all, 4 CTAs = 16 warps per SM, which measured faster
+// than the 20 warps of a 96-register build that fetched the emit pass's candidate tile without the look-ahead.  A second set of
+// shared-memory tiles would cost 5.4 KB per warp.
+// tile t of a 32-bit-per-position array: 32 coalesced 128-byte rows, all issued at once.  base = the block's array, bn = positions in the block
+__device__ __forceinline__ void dp_fetch_cand(uint32_t (&r)[32], const uint32_t* __restrict__ base, uint32_t bn, uint32_t t, uint32_t lane) {
+#pragma unroll
     for (uint32_t j = 0; j < 32u; j++) {
         const uint32_t pos = j * B2Z_SEG + 32u * t + lane;
-        sm.candTile[j][lane] = pos < bn ? __ldcs(base + pos) : 0u;
+        r[j] = pos < bn ? __ldcs(base + pos) : 0u;
     }
 }
-// tile t of a byte-per-position array: 8 loads of 4 rows x 32 bytes
-__device__ __forceinline__ void dp_load_byte_tile(uint32_t (*tile)[9], const uint8_t* __restrict__ base, uint32_t bn, uint32_t t, uint32_t lane) {
+__device__ __forceinline__ void dp_put_cand(DpWarpSmem& sm, const uint32_t (&r)[32], uint32_t lane) {
 #pragma unroll
-    for (uint32_t r = 0; r < 8u; r++) {
-        const uint32_t row = 4u * r + (lane >> 3), wd = lane & 7u, pos = row * B2Z_SEG + 32u * t + 4u * wd;
-        tile[row][wd] = pos < bn ? __ldg(reinterpret_cast<const uint32_t*>(base + pos)) : 0u;
+    for (uint32_t j = 0; j < 32u; j++) sm.candTile[j][lane] = r[j];
+}
+// tile t of a byte-per-position array: 8 loads of 4 rows x 32 bytes
+__device__ __forceinline__ void dp_fetch_bytes(uint32_t (&r)[8], const uint8_t* __restrict__ base, uint32_t bn, uint32_t t, uint32_t lane) {
+#pragma unroll
+    for (uint32_t k = 0; k < 8u; k++) {
+        const uint32_t row = 4u * k + (lane >> 3), wd = lane & 7u, pos = row * B2Z_SEG + 32u * t + 4u * wd;
+        r[k] = pos < bn ? __ldg(reinterpret_cast<const uint32_t*>(base + pos)) : 0u;
     }
+}
+__device__ __forceinline__ void dp_put_bytes(uint32_t (*tile)[9], const uint32_t (&r)[8], uint32_t lane) {
+#pragma unroll
+    for (uint32_t k = 0; k < 8u; k++) tile[4u * k + (lane >> 3)][lane & 7u] = r[k];
 }
 __device__ __forceinline__ void dp_store_byte_tile(const uint32_t (*tile)[9], uint8_t* __restrict__ base, uint32_t bn, uint32_t t, uint32_t lane) {
 #pragma unroll
@@ -71,6 +98,26 @@ __device__ __forceinline__ void dp_store_byte_tile(const uint32_t (*tile)[9], ui
         const uint32_t row = 4u * r + (lane >> 3), wd = lane & 7u, pos = row * B2Z_SEG + 32u * t + 4u * wd;
         if (pos < bn) *reinterpret_cast<uint32_t*>(base + pos) = tile[row][wd];
     }
+}
+
+// The match half of step p of the programme (p = position in the tile): the candidate priced at its length L, L-1 .. L-NTRUNC as
+// (price << 2 | k), minimum over the lengths that qualify, so a tie goes to the longer one as in the sequential statement's strict
+// '<' tests.  mc = the price (2^30 - 1 when no length qualifies: more than any literal path), mh = the length.  Positions past the
+// segment end (p >= lim) get price 0 and length 0, which makes the step's cost 0 -- the end's cost -- and its choice a literal.
+static_assert(DP_RING == 32u && B2Z_DP_NTRUNC < 4u && (uint64_t)B2Z_SEG * B2Z_DP_LIT_MAX + 1024u < (1u << 29),
+              "ring slot = position in the tile; k fits two bits; a cost fits 29 bits");
+__device__ __forceinline__ void dp_match(const DpWarpSmem& sm, uint32_t lane, uint32_t p, uint32_t lim, uint32_t& mc, uint32_t& mh) {
+    const uint32_t c = sm.candTile[lane][p];
+    const uint32_t len = B2Z_CAND_LEN(c), ob = 16u * highbit32(B2Z_CAND_OFF(c) + 3u) + B2Z_DP_MATCH;
+    uint32_t m = 0xFFFFFFFFu;
+#pragma unroll
+    for (uint32_t k = 0; k <= B2Z_DP_NTRUNC; k++) {
+        // wraps below zero when len < k: the index stays inside the ring, the price is discarded
+        const uint32_t key = ((ob + sm.ring[(p + len - k) & (DP_RING - 1u)][lane]) << 2) | k;
+        m = (len >= B2Z_DP_MINLEN + k && key < m) ? key : m;
+    }
+    mc = p >= lim ? 0u : m >> 2;
+    mh = p >= lim ? 0u : len - (m & 3u);
 }
 
 // per-lane state of the forward walk over a segment's choices
@@ -94,14 +141,16 @@ __device__ __forceinline__ uint32_t dp_nonzero_mask(const uint32_t* row) {
 
 // one tile of the forward walk: positions [32 t, 32 t + 32) of the lane's segment, as far as the lane's path touches them.  On the
 // path, literals are exactly the positions up to the next non-zero choice, so a whole literal run is one iteration (find-first-set on
-// the tile's "choice != 0" mask), and the loop runs once per match instead of once per position.
+// the tile's "choice != 0" mask), and the loop runs once per match instead of once per position.  EMIT: returns the tile's positions
+// that are literals of the path (bit w = position 32 t + w), which dp_emit_literals writes out.
 template <bool EMIT>
-__device__ __forceinline__ void dp_walk_tile(DpWarpSmem& sm, DpWalk& k, uint32_t t, uint32_t lane, uint32_t sn, uint32_t s0 /* block-relative */,
+__device__ __forceinline__ uint32_t dp_walk_tile(DpWarpSmem& sm, DpWalk& k, uint32_t t, uint32_t lane, uint32_t sn, uint32_t s0 /* block-relative */,
                                              const uint64_t* __restrict__ fw /* frame as words */, uint32_t segAbs /* frame-relative */, uint32_t nWords,
                                              const uint32_t* __restrict__ cnd /* segment's candidate words */,
-                                             uint64_t* __restrict__ outSeq, uint8_t* __restrict__ outLit) {
+                                             uint64_t* __restrict__ outSeq) {
     const uint32_t tEnd = (32u * t + 32u) < sn ? (32u * t + 32u) : sn;
-    if (k.i >= tEnd) return;
+    uint32_t lits = 0;
+    if (k.i >= tEnd) return lits;
     const uint32_t inTile = tEnd - 32u * t;
     const uint32_t M = dp_nonzero_mask(sm.chcTile[lane]) & (inTile >= 32u ? 0xFFFFFFFFu : ((1u << inTile) - 1u));
     while (k.i < tEnd) {
@@ -109,7 +158,7 @@ __device__ __forceinline__ void dp_walk_tile(DpWarpSmem& sm, DpWalk& k, uint32_t
         const uint32_t rem = M >> w;
         const uint32_t r = rem ? (uint32_t)(__ffs((int)rem) - 1) : (tEnd - k.i);        // literals up to the next match of the tile (or the tile's end)
         if (r) {
-            if (EMIT) for (uint32_t j = 0; j < r; j++) { const uint32_t ww = w + j; outLit[k.nl + j] = (uint8_t)(sm.srcTile[lane][ww >> 2] >> (8u * (ww & 3u))); }
+            if (EMIT) lits |= (0xFFFFFFFFu >> (32u - r)) << w;
             k.nl += r; k.i += r; w += r;
             if (!rem) break;
         }
@@ -139,6 +188,18 @@ __device__ __forceinline__ void dp_walk_tile(DpWarpSmem& sm, DpWalk& k, uint32_t
         }
         k.ns++; k.i += l; k.lastEnd = s0 + k.i;
     }
+    return lits;
+}
+
+// the literals of one tile, lane by lane: lane L's are the bytes of its source row where bit `lits` is set, due at out + dst (its
+// place in the block's literal array); lane j of the warp writes byte j when it is one, so each store covers one lane's run in
+// one or two sectors instead of 32 lanes' bytes in 32 lines.  The source rows must be in shared memory (synced).
+__device__ __forceinline__ void dp_emit_literals(const DpWarpSmem& sm, uint32_t lits, uint32_t dst, uint32_t lane, uint8_t* __restrict__ out) {
+    const uint32_t below = (1u << lane) - 1u;
+    for (uint32_t L = 0; L < 32u; L++) {
+        const uint32_t m = __shfl_sync(B2Z_FULL, lits, L), d = __shfl_sync(B2Z_FULL, dst, L);
+        if (m >> lane & 1u) out[d + __popc(m & below)] = (uint8_t)(sm.srcTile[L][lane >> 2] >> (8u * (lane & 3u)));
+    }
 }
 
 __global__ void __launch_bounds__(B2Z_DP_WARPS * 32)
@@ -165,6 +226,10 @@ zstd_enc_dp_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
     uint64_t* __restrict__ out = seqs + (size_t)bw * B2Z_MAXSEQ;
     uint8_t* __restrict__ lit = lits + f0 + b0;
     const uint32_t nTiles = ((bn < B2Z_SEG ? bn : B2Z_SEG) + 31u) >> 5;        // tiles of the longest segment (the first)
+#ifdef B2Z_DP_CLOCKS
+    unsigned long long dpc[DPC_N] = {};
+    long long dpLast = clock64();
+#endif
 
     // ---- 1. literal prices
     uint32_t* const hist = &sm.candTile[0][0];
@@ -197,6 +262,7 @@ zstd_enc_dp_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
         }
     }
     __syncwarp();
+    DP_TICK(DPC_HIST);
 
     // ---- 2. backward dynamic programme, tile by tile from the segment's end
     const uint32_t s0 = lane * B2Z_SEG;
@@ -204,60 +270,70 @@ zstd_enc_dp_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
     const uint32_t sn = active ? ((bn - s0) < B2Z_SEG ? (bn - s0) : B2Z_SEG) : 0u;
     uint32_t diff = 0;                                                         // any byte of the segment unlike the block's first byte
     const uint32_t first = bs[0];
+    const uint32_t first4 = first * 0x01010101u;
+    uint32_t c1 = 0;                                                           // cost[i + 1]: 0 at the segment's end
     if (active) sm.ring[sn & (DP_RING - 1u)][lane] = 0;
+    uint32_t cr[32], sr[8];                                                    // the next tile's loads
+    dp_fetch_cand(cr, cndB, bn, nTiles - 1u, lane);
+    dp_fetch_bytes(sr, bs, bn, nTiles - 1u, lane);
     for (uint32_t t = nTiles; t-- > 0;) {
-        dp_load_cand_tile(sm, cndB, bn, t, lane);
-        dp_load_byte_tile(sm.srcTile, bs, bn, t, lane);
+        dp_put_cand(sm, cr, lane);
+        dp_put_bytes(sm.srcTile, sr, lane);
+        if (t) { dp_fetch_cand(cr, cndB, bn, t - 1u, lane); dp_fetch_bytes(sr, bs, bn, t - 1u, lane); }
         __syncwarp();
+        DP_TICK(DPC_DP_LOAD);
         if (32u * t < sn) {
-            const bool full = 32u * t + 32u <= sn;                             // only the last tile of a short segment is not
+            // Each step is cost[i] = min(literal + cost[i + 1], the match price), with cost[i + 1] in a register.  The match price
+            // only reads cost[i + B2Z_DP_MINLEN ..], so it is formed four positions ahead (mc, mh: price and length), right after
+            // the cost it needs last was stored, and its ring loads are in flight while the chain runs three more steps.
+            const uint32_t lim = sn - 32u * t;                                 // positions of the tile in the segment (>= 32: all)
+            uint32_t mc[4], mh[4];                                             // [j]: position 4 wi + 3 - j
+#pragma unroll
+            for (uint32_t j = 0; j < 4u; j++) dp_match(sm, lane, 31u - j, lim, mc[j], mh[j]);
 #pragma unroll 2
             for (int wi = 7; wi >= 0; wi--) {
                 const uint32_t b4 = sm.srcTile[lane][wi];
+                const int inWord = (int)lim - 4 * wi;                          // bytes of the word inside the segment
+                const uint32_t x = b4 ^ first4;
+                diff |= inWord >= 4 ? x : (inWord > 0 ? x & ((1u << (8 * inWord)) - 1u) : 0u);
                 uint32_t packed = 0;
 #pragma unroll
-                for (int j = 3; j >= 0; j--) {
-                    const uint32_t i = 32u * t + 4u * (uint32_t)wi + (uint32_t)j;
-                    if (!full && i >= sn) continue;
-                    // branch-free: an absent or too short candidate prices at 2^31 and loses against the literal
-                    const uint32_t byte = (b4 >> (8 * j)) & 255u;
-                    diff |= byte ^ first;
-                    const uint32_t c = sm.candTile[lane][4 * wi + j];
-                    const uint32_t len = B2Z_CAND_LEN(c), ob = 16u * highbit32(B2Z_CAND_OFF(c) + 3u) + B2Z_DP_MATCH;
-                    uint32_t best = (uint32_t)sm.litc[byte] + sm.ring[(i + 1u) & (DP_RING - 1u)][lane], ch = 0;
-#pragma unroll
-                    for (uint32_t k = 0; k <= B2Z_DP_NTRUNC; k++) {
-                        const uint32_t l = len - k;                            // wraps below zero when len < k: the index stays inside the ring, the price is discarded
-                        const uint32_t pr = ob + sm.ring[(i + l) & (DP_RING - 1u)][lane];
-                        const bool take = (len >= B2Z_DP_MINLEN + k) && pr < best;
-                        best = take ? pr : best; ch = take ? l : ch;
-                    }
-                    sm.ring[i & (DP_RING - 1u)][lane] = best;
-                    packed |= ch << (8 * j);
+                for (uint32_t j = 0; j < 4u; j++) {
+                    const uint32_t p = 4u * (uint32_t)wi + 3u - j, sh = 8u * (3u - j);
+                    const uint32_t lc = c1 + sm.litc[(b4 >> sh) & 255u];
+                    c1 = lc < mc[j] ? lc : mc[j];                              // the literal wins a tie
+                    packed |= (mc[j] < lc ? mh[j] : 0u) << sh;
+                    sm.ring[p][lane] = c1;                                     // p = i & (DP_RING - 1)
+                    if (wi > 0) dp_match(sm, lane, p - 4u, lim, mc[j], mh[j]);
                 }
                 sm.chcTile[lane][wi] = packed;
             }
         }
         __syncwarp();
+        DP_TICK(DPC_DP);
         dp_store_byte_tile(sm.chcTile, chcB, bn, t, lane);
-        __syncwarp();
+        DP_TICK(DPC_DP_STORE);
     }
     // ---- one repeated byte: the canonical single sequence (stage E emits an RLE block for it)
     if (!__any_sync(B2Z_FULL, diff != 0u) && bn > 1u) {
         if (lane == 0) { out[0] = B2Z_PACK_SEQ(1u + 3u, 1u, bn - 1u); lit[0] = bs[0]; nseq[bw] = 1u; nlit[bw] = 1u; }
+        DP_CLOCKS_FLUSH();
         return;
     }
 
     const uint64_t* __restrict__ fw = reinterpret_cast<const uint64_t*>(fb);
     const uint32_t nWords = (n + 7u) >> 3;
     const uint32_t* __restrict__ cnd = cndB + s0;
-    // ---- 3. count
+    // ---- 3. count (tile 0's choices are still in shared memory from the last step of the programme: each lane's own row)
     DpWalk k; k.i = 0; k.ns = 0; k.nl = 0; k.lastEnd = 0; k.rep0 = k.rep1 = k.rep2 = 0; k.prevEnd = 0;
+    uint32_t qr[8];
     for (uint32_t t = 0; t < nTiles; t++) {
-        dp_load_byte_tile(sm.chcTile, chcB, bn, t, lane);
+        if (t) { dp_put_bytes(sm.chcTile, qr, lane); __syncwarp(); }
+        if (t + 1u < nTiles) dp_fetch_bytes(qr, chcB, bn, t + 1u, lane);
+        DP_TICK(DPC_CNT_LOAD);
+        dp_walk_tile<false>(sm, k, t, lane, sn, s0, fw, b0 + s0, nWords, cnd, nullptr);
         __syncwarp();
-        dp_walk_tile<false>(sm, k, t, lane, sn, s0, fw, b0 + s0, nWords, cnd, nullptr, nullptr);
-        __syncwarp();
+        DP_TICK(DPC_CNT);
     }
     const uint32_t cntSeq = k.ns, cntLit = k.nl;
     // ---- 4. places: exclusive sums of the counts, exclusive maximum of the last match ends
@@ -270,17 +346,27 @@ zstd_enc_dp_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
     const uint32_t totSeq = __shfl_sync(B2Z_FULL, seqBase, 31), totLit = __shfl_sync(B2Z_FULL, litBase, 31);
     seqBase -= cntSeq; litBase -= cntLit;
     prevEnd = __shfl_up_sync(B2Z_FULL, prevEnd, 1); if (lane == 0) prevEnd = 0;
+    DP_TICK(DPC_SCAN);
     // ---- 5. emit
     k.i = 0; k.ns = 0; k.nl = 0; k.prevEnd = prevEnd;
+    dp_fetch_bytes(qr, chcB, bn, 0, lane);
+    dp_fetch_bytes(sr, bs, bn, 0, lane);
+    dp_fetch_cand(cr, cndB, bn, 0, lane);
     for (uint32_t t = 0; t < nTiles; t++) {
-        dp_load_byte_tile(sm.chcTile, chcB, bn, t, lane);
-        dp_load_byte_tile(sm.srcTile, bs, bn, t, lane);
-        dp_load_cand_tile(sm, cndB, bn, t, lane);
+        dp_put_bytes(sm.chcTile, qr, lane);
+        dp_put_bytes(sm.srcTile, sr, lane);
+        dp_put_cand(sm, cr, lane);
+        if (t + 1u < nTiles) { dp_fetch_bytes(qr, chcB, bn, t + 1u, lane); dp_fetch_bytes(sr, bs, bn, t + 1u, lane); dp_fetch_cand(cr, cndB, bn, t + 1u, lane); }
         __syncwarp();
-        dp_walk_tile<true>(sm, k, t, lane, sn, s0, fw, b0 + s0, nWords, cnd, out + seqBase, lit + litBase);
+        DP_TICK(DPC_EMIT_LOAD);
+        const uint32_t litAt = litBase + k.nl;
+        const uint32_t lits = dp_walk_tile<true>(sm, k, t, lane, sn, s0, fw, b0 + s0, nWords, cnd, out + seqBase);
+        dp_emit_literals(sm, lits, litAt, lane, lit);
         __syncwarp();
+        DP_TICK(DPC_EMIT);
     }
     if (lane == 0) { nseq[bw] = totSeq; nlit[bw] = totLit; }
+    DP_CLOCKS_FLUSH();
 }
 
 #ifndef B2Z_CUEMU
@@ -296,6 +382,16 @@ cudaError_t launch_zstd_enc_dp(const uint8_t* src, uint64_t srcSize, const EncGe
     zstd_enc_dp_kernel<<<(nBlockSlots + B2Z_DP_WARPS - 1) / B2Z_DP_WARPS, B2Z_DP_WARPS * 32, zstd_enc_dp_smem_bytes(), st>>>(
         src, srcSize, g, cand, choice, seqs, nseq, lits, nlit, nBlockSlots);
     return cudaGetLastError();
+}
+#endif
+
+#if defined(B2Z_DP_CLOCKS) && !defined(B2Z_CUEMU)
+// the per-phase cycle sums of every warp since the last call (DPC_* order, then the warp count); clears them
+extern "C" int b200z_dp_clocks(unsigned long long* out) {
+    static const unsigned long long zero[DPC_N + 1] = {};
+    cudaError_t e = cudaMemcpyFromSymbol(out, dp_clocks, sizeof(dp_clocks));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(dp_clocks, zero, sizeof(dp_clocks));
+    return (int)e;
 }
 #endif
 
