@@ -21,7 +21,7 @@ EXPORTS = [
     "b200z_last_error", "b200z_get_stat", "b200z_reset_stats", "b200z_zstd_compress_bound",
     "b200z_zstd_compress_device", "b200z_zstd_compress_host", "b200z_zstd_frame_info",
     "b200z_zstd_decompress_device", "b200z_zstd_decompress_host", "b200z_zstd_enc_stage_m", "b200z_zstd_enc_stage_f",
-    "b200z_dev_alloc", "b200z_dev_free", "b200z_dev_upload", "b200z_dev_download",
+    "b200z_zstd_enc_stage_e", "b200z_dev_alloc", "b200z_dev_free", "b200z_dev_upload", "b200z_dev_download",
     "b200z_host_alloc_pinned", "b200z_host_free_pinned",
 ]
 
@@ -64,6 +64,7 @@ def load_library():
     L.b200z_zstd_frame_info.argtypes = [vp, sz, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint32)]
     L.b200z_zstd_enc_stage_m.argtypes = [vp, vp, sz, vp, vp, vp, vp]
     L.b200z_zstd_enc_stage_f.argtypes = [vp, vp, sz, vp]
+    L.b200z_zstd_enc_stage_e.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]
     L.b200z_zstd_compress_batch_bound.argtypes = [vp, sz, ctypes.c_uint32]; L.b200z_zstd_compress_batch_bound.restype = sz
     L.b200z_zstd_compress_batch_host.argtypes = [vp, vp, vp, ctypes.c_uint32, vp, sz, vp]
     L.b200z_zstd_compress_batch_crc_host.argtypes = [vp, vp, vp, ctypes.c_uint32, vp, sz, vp, vp]
@@ -317,6 +318,28 @@ class Codec:
         finally:
             self.L.b200z_dev_free(self.h, d)
         return cand
+
+    # ---- test tap: stage E alone on given sequences and literals (layout of oracle b2zo_zstd_find_sequences) -> (the coded
+    # blocks back to back, their sizes)
+    def stage_e(self, src, seqs, nseq, lits, nlit):
+        import numpy as np
+        src = np.frombuffer(src, dtype=np.uint8) if isinstance(src, (bytes, bytearray, memoryview)) else src
+        n = src.nbytes
+        nblk = (n + 131071) // 131072
+        seqs = np.ascontiguousarray(seqs, dtype=np.uint64); nseq = np.ascontiguousarray(nseq, dtype=np.uint32)
+        lits = np.ascontiguousarray(lits, dtype=np.uint8); nlit = np.ascontiguousarray(nlit, dtype=np.uint32)
+        if seqs.size < nblk * MAXSEQ or nseq.size < nblk or lits.size < n or nlit.size < nblk:
+            raise ValueError("stage_e: arrays smaller than the block layout of the source")
+        out = np.empty(n + 3 * nblk, dtype=np.uint8); sizes = np.zeros(nblk, dtype=np.uint32)
+        d = ctypes.c_void_p()
+        self._check(self.L.b200z_dev_alloc(self.h, ctypes.byref(d), n + 64))
+        try:
+            self._check(self.L.b200z_dev_upload(self.h, d, src.ctypes.data, n))
+            self._check(self.L.b200z_zstd_enc_stage_e(self.h, d, n, seqs.ctypes.data, nseq.ctypes.data, lits.ctypes.data, nlit.ctypes.data,
+                                                      out.ctypes.data, out.nbytes, sizes.ctypes.data))
+        finally:
+            self.L.b200z_dev_free(self.h, d)
+        return out[:int(sizes.sum(dtype=np.uint64))].tobytes(), sizes
 
     # ---- test tap: the price-based LZMA2 parse (lzma2_parse=1): stage C candidate words [n, 4] and stage P sequences
     # (layouts of the oracle's b2zo_lzma2_candidates / b2zo_lzma2_parse_frame, frames back to back)

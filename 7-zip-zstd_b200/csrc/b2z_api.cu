@@ -513,6 +513,56 @@ int b200z_zstd_enc_stage_m(b200z_ctx* ctx, const void* d_src, size_t srcSize, ui
     return 0;
 }
 
+// Stage E alone on sequences and literals the caller built: the host arrays in the oracle's dense block layout go to the per-frame
+// block stride (the inverse of stage_m's copy), and stage E is launched as enc_batch launches it.  The slots and the scratch are
+// filled with 0xCD first, so that a byte stage E reads without having written it shows up in the output.
+int b200z_zstd_enc_stage_e(b200z_ctx* ctx, const void* d_src, size_t srcSize, const uint64_t* seqs, const uint32_t* nseq,
+                           const uint8_t* lits, const uint32_t* nlit, void* dst, size_t dstCap, uint32_t* slotSize) {
+    if (!ctx || !d_src || !srcSize || !seqs || !nseq || !lits || !nlit || !dst || !slotSize) return B200Z_E_PARAM;
+    CU(cudaSetDevice(ctx->device));
+    const uint64_t F = 1ull << ctx->geom.frameLog; const uint32_t bpf = (uint32_t)(F >> 17);
+    const uint64_t nFrames = (srcSize + F - 1) / F;
+    const uint32_t nBlocks = (uint32_t)((srcSize + B2Z_BLOCK - 1) / B2Z_BLOCK);
+    uint64_t need = 0;
+    for (uint32_t b = 0; b < nBlocks; b++) {
+        const uint64_t bn = (srcSize - (uint64_t)b * B2Z_BLOCK) < B2Z_BLOCK ? (srcSize - (uint64_t)b * B2Z_BLOCK) : B2Z_BLOCK;
+        if (nseq[b] > B2Z_MAXSEQ || nlit[b] > bn) return fail(ctx, B200Z_E_PARAM, "stage E: a block has more sequences or literals than it can hold%s");
+        need += bn + 3;
+    }
+    if (dstCap < need) return fail(ctx, B200Z_E_DSTSIZE, "stage E: dstCap < the blocks' raw sizes + 3 each%s");
+    int rc = enc_reserve(ctx, srcSize);
+    if (rc) return rc;
+    cudaStream_t st = ctx->stream;
+    CU(cudaMemsetAsync(ctx->slots.p, 0xCD, (size_t)nBlocks * B2Z_SLOT, st));
+    CU(cudaMemsetAsync(ctx->slotSize.p, 0xCD, (size_t)nBlocks * 4, st));
+    CU(cudaMemsetAsync(ctx->cand.p, 0xCD, ctx->cand.cap, st));
+    uint64_t dense = 0;
+    for (uint64_t f = 0; f < nFrames; f++) {
+        const uint64_t fn = (srcSize - f * F) < F ? (srcSize - f * F) : F;
+        const uint32_t nb = (uint32_t)((fn + B2Z_BLOCK - 1) / B2Z_BLOCK);
+        const size_t sb = (size_t)f * bpf;
+        CU(cudaMemcpyAsync((uint32_t*)ctx->nseq.p + sb, nseq + dense, nb * 4, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync((uint32_t*)ctx->nlit.p + sb, nlit + dense, nb * 4, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync((uint64_t*)ctx->seqs.p + sb * B2Z_MAXSEQ, seqs + dense * B2Z_MAXSEQ, (size_t)nb * B2Z_MAXSEQ * 8, cudaMemcpyHostToDevice, st));
+        dense += nb;
+    }
+    CU(cudaMemcpyAsync(ctx->lits.p, lits, srcSize, cudaMemcpyHostToDevice, st));
+    launch_zstd_enc_entropy((const uint8_t*)d_src, srcSize, ctx->geom, (const uint64_t*)ctx->seqs.p, (const uint32_t*)ctx->nseq.p, (const uint8_t*)ctx->lits.p,
+                            (const uint32_t*)ctx->nlit.p, (uint8_t*)ctx->slots.p, (uint32_t*)ctx->slotSize.p, (uint8_t*)ctx->cand.p,
+                            nBlocks, ctx->smCount, st);
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(st));
+    CU(cudaMemcpy(slotSize, ctx->slotSize.p, (size_t)nBlocks * 4, cudaMemcpyDeviceToHost));
+    uint8_t* out = (uint8_t*)dst;
+    for (uint32_t b = 0; b < nBlocks; b++) {                        // the slots back to back, in block order
+        const uint64_t bn = (srcSize - (uint64_t)b * B2Z_BLOCK) < B2Z_BLOCK ? (srcSize - (uint64_t)b * B2Z_BLOCK) : B2Z_BLOCK;
+        if (slotSize[b] > bn + 3) return fail(ctx, B200Z_E_CUDA, "stage E: a slot is larger than its raw block%s");
+        CU(cudaMemcpy(out, (const uint8_t*)ctx->slots.p + (size_t)b * B2Z_SLOT, slotSize[b], cudaMemcpyDeviceToHost));
+        out += slotSize[b];
+    }
+    return 0;
+}
+
 int b200z_zstd_enc_stage_f(b200z_ctx* ctx, const void* d_src, size_t srcSize, uint32_t* cand) {
     if (!ctx || !d_src || !srcSize || !cand) return B200Z_E_PARAM;
     if (price_parse(ctx->geom, 0)) return fail(ctx, B200Z_E_PARAM, "stage F belongs to B200Z_P_ZSTD_PARSE 0%s");

@@ -149,6 +149,12 @@ int b200z_zstd_decompress_host(b200z_ctx *ctx, const void *src, size_t srcSize,
 int b200z_zstd_enc_stage_m(b200z_ctx *ctx, const void *d_src, size_t srcSize,
                            uint64_t *seqs, uint32_t *nseq, uint8_t *lits, uint32_t *nlit);
 int b200z_zstd_enc_stage_f(b200z_ctx *ctx, const void *d_src, size_t srcSize, uint32_t *cand);
+/* stage_e: stage E (the entropy coder) alone, on the device buffer d_src and per-block sequences and literals from host arrays in
+ * the layout of b2zo_zstd_find_sequences (seqs[b * 32768 + i] packed by B2Z_PACK_SEQ, block b's literals at lits + b * 128 KiB);
+ * the finished blocks (3-byte header included) are written to dst back to back, their sizes to slotSize[b].  dstCap must cover
+ * every block's raw size + 3. */
+int b200z_zstd_enc_stage_e(b200z_ctx *ctx, const void *d_src, size_t srcSize, const uint64_t *seqs, const uint32_t *nseq,
+                           const uint8_t *lits, const uint32_t *nlit, void *dst, size_t dstCap, uint32_t *slotSize);
 
 /* ---- non-solid .7z archives of many files in one pass (BASELINE configs[4]; csrc/sevenz_api.cu) ----------------------------------
  * The reference's archive layer runs one Code() per file, strictly one after the other (CPP/7zip/Archive/7z/7zUpdate.cpp:2739-2810,

@@ -45,6 +45,12 @@ int64_t b2zo_zstd_find_sequences(const void *src, size_t srcSize, const b2zo_enc
                                  uint64_t *seqs /* [nblocks*B2Z_MAXSEQ] */, uint32_t *nseq /* [nblocks] */,
                                  uint8_t *lits /* [srcSize] */, uint32_t *nlit /* [nblocks] */);
 
+/* Stage tap for parity with the GPU's stage E: one block [blkStart, blkStart + blkSize) of `frame` coded from its sequences
+ * (B2Z_PACK_SEQ) and literal bytes, with its 3-byte header (last = Last_Block flag).  Returns the bytes written (at most
+ * blkSize + 3), -1 on a bad argument, -2 when dstCap < blkSize + 3. */
+int64_t b2zo_zstd_encode_block(void *dst, size_t dstCap, const void *frame, size_t blkStart, size_t blkSize, int last,
+                               const uint64_t *seqs, uint32_t nbSeq, const uint8_t *lits, uint32_t nlit);
+
 
 /* ---- LZMA2 (method 21) decoder: lzma2_dec_oracle.c ---- */
 /* raw LZMA2 chunk stream -> dst; dictProp = the coder's 1-byte property. returns size, -1 corrupt, -2 dst too small */

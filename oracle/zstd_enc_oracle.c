@@ -645,6 +645,13 @@ static size_t compress_block(uint8_t *dst, const uint8_t *frame, size_t blkStart
     return out;
 }
 
+int64_t b2zo_zstd_encode_block(void *dst, size_t dstCap, const void *frame, size_t blkStart, size_t blkSize, int last,
+                               const uint64_t *seqs, uint32_t nbSeq, const uint8_t *lits, uint32_t nlit) {
+    if (blkSize == 0 || blkSize > ZF_BLOCK_MAX || nbSeq > B2Z_MAXSEQ || nlit > blkSize) return -1;
+    if (dstCap < blkSize + 3) return -2;                    /* a block is never larger than its raw form */
+    return (int64_t)compress_block((uint8_t *)dst, (const uint8_t *)frame, blkStart, blkSize, last, seqs, nbSeq, lits, nlit);
+}
+
 static size_t write_frame_header(uint8_t *dst, size_t n, const b2zo_enc_params *P) {
     wr32(dst, ZF_MAGIC);
     if (n == 0) { dst[4] = (uint8_t)(0x20 | ((P->flags & 2) ? 4 : 0)); dst[5] = 0; return 6; }     /* single segment, FCS = 0 */
