@@ -456,29 +456,68 @@ __device__ void huf_fill(uint16_t* huf, const uint8_t* w, uint32_t nw, uint32_t 
 // Hot-loop reader (32-bit arithmetic): `cont` holds stream bytes [bytePos, bytePos+8); the next unread bit is
 // bit (63 - consumed) of it.  After reload() consumed <= 7, so 57 bits can be read before the next reload.
 // Bytes below the stream start read as zero; left() < 0 means the stream was over-read.
+//
+// No reload waits for memory.  `cont` is built with a funnel shift from the two aligned source words that hold it (lo = word wi,
+// hi = word wi + 1, in registers).  The B2Z_BWD_DEPTH words below them are in flight to the thread's ring in shared memory
+// (`ring`, B2Z_BWD_DEPTH words, word k in slot k mod B2Z_BWD_DEPTH): when the window crosses into the next word down, that word is
+// taken from the ring and the one B2Z_BWD_DEPTH further down is asked for (cp.async, zero-filled for indices outside the source,
+// which are never read).  A load is so first used about B2Z_BWD_DEPTH * 8 stream bytes after it was issued.  A reader's words
+// still in flight are waited for by its next init() and by drain().
+#define B2Z_BWD_DEPTH 4u
 struct FastBwd {
-    const Src* S; uint64_t base; uint64_t cont; int32_t bytePos; uint32_t consumed;
-    __device__ __forceinline__ uint64_t fetch() const {
-        if (bytePos >= 0) return S->le64(base + (uint32_t)bytePos);
-        if (bytePos > -8) return S->le64(base) << ((uint32_t)(-bytePos) * 8u);
-        return 0ull;
+    const Src* S; uint64_t* ring; uint64_t cont, lo, hi; int64_t wi; int32_t bytePos; uint32_t consumed, o;     // o = (start of cont) & 7
+    __device__ __forceinline__ uint64_t word(int64_t k) const { return k >= 0 ? S->word((uint64_t)k) : 0ull; }
+    __device__ __forceinline__ void issue(int64_t k) {                                      // word k into its ring slot
+        uint64_t* d = ring + ((uint32_t)k & (B2Z_BWD_DEPTH - 1u));
+#ifndef B2Z_CUEMU
+        const bool in = k >= 0 && (uint64_t)k < S->nWords;
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;\n\tcp.async.commit_group;" ::
+                     "r"((uint32_t)__cvta_generic_to_shared(d)), "l"(S->w + (in ? k : 0)), "r"(in ? 8u : 0u) : "memory");
+#else
+        *d = word(k);
+#endif
     }
-    __device__ __forceinline__ int init(const Src* s, uint64_t b, uint32_t size) {
-        S = s; base = b;
+    __device__ __forceinline__ void drain() const {
+#ifndef B2Z_CUEMU
+        asm volatile("cp.async.wait_all;" ::: "memory");
+#endif
+    }
+    __device__ __forceinline__ void window() {                                              // cont from lo, hi; zero below the start
+        cont = funnel64(lo, hi, o * 8u);
+        if (bytePos < 0) cont = bytePos > -8 ? cont & (~0ull << ((uint32_t)(-bytePos) * 8u)) : 0ull;
+    }
+    __device__ __forceinline__ int init(const Src* s, uint64_t* r, uint64_t b, uint32_t size) {
+        S = s; ring = r;
         if (!size) return -1;
         const uint32_t lastByte = S->u8(b + size - 1);
         if (!lastByte) return -1;
         bytePos = (int32_t)size - 8; consumed = 8u - highbit32(lastByte);      // skip the padding and the end mark
-        cont = fetch();
+        const int64_t p = (int64_t)b + bytePos;
+        wi = p >> 3; o = (uint32_t)p & 7u;
+        drain();                                                                // the ring's slots are free
+        lo = word(wi); hi = word(wi + 1);
+        for (uint32_t d = 1; d <= B2Z_BWD_DEPTH; d++) issue(wi - d);
+        window();
         return 0;
     }
-    // The stream is read downwards: the line 256 bytes below is asked into L2 now, so that the reload that reaches it does not wait
-    // for HBM (one such wait per 128 bytes was the largest part of a stream's time).
+    // The line 256 bytes below is also asked into L2 when a word is crossed, so that the ring's load that reaches it does not wait for
+    // HBM.
     __device__ __forceinline__ void reload() {
-        bytePos -= (int32_t)(consumed >> 3); consumed &= 7u; cont = fetch();
+        const uint32_t d = consumed >> 3;                                       // <= 8 bytes: at most one word is crossed
+        bytePos -= (int32_t)d; consumed &= 7u;
+        if (o < d) {
 #ifndef B2Z_CUEMU
-        if (bytePos >= 256) asm volatile("prefetch.L2 [%0];" :: "l"(S->w + ((base + (uint32_t)bytePos - 256u) >> 3)));
+            asm volatile("cp.async.wait_group %0;" :: "n"(B2Z_BWD_DEPTH - 1u) : "memory");    // word wi - 1 has arrived
 #endif
+            wi--; hi = lo; lo = ring[(uint32_t)wi & (B2Z_BWD_DEPTH - 1u)];
+            issue(wi - (int64_t)B2Z_BWD_DEPTH);
+#ifndef B2Z_CUEMU
+            if (bytePos >= 256 + 8) asm volatile("prefetch.L2 [%0];" :: "l"(S->w + (wi - 32)));
+#endif
+            o += 8u;
+        }
+        o -= d;
+        window();
     }
     __device__ __forceinline__ uint32_t read(uint32_t n) {                      // n <= 32 (0 allowed)
         const uint32_t v = (uint32_t)(((cont << consumed) >> 1) >> (63u - n));
@@ -498,6 +537,21 @@ struct FastBwd {
 // Each serial bitstream is decoded by ONE THREAD, so that thousands of dependent chains overlap.  A table is built from the
 // description in src (an earlier block's for treeless literals and repeat mode: any block may be read, a CTA depends on no other
 // CTA).  The stream kernels loop over their groups of blocks, so they do not depend on the grid they are given.
+// -DB2Z_D1_CLOCKS (off by default; tools/dec_entropy_profile.py --build-clocks): every stream thread of the two stream kernels
+// adds the clock64() cycles it spends in each phase -- table build, refills, table look-ups and arithmetic, output stores -- to
+// d1_clocks[]; b200z_d1_clocks() reads and clears them.  Without the switch the ticks compile to nothing.
+enum { D1C_TABLE, D1C_REFILL, D1C_DECODE, D1C_STORE, D1C_N };
+#ifdef B2Z_D1_CLOCKS
+__device__ unsigned long long d1_clocks[2 * D1C_N];                     // literal kernel's phases, then the sequence kernel's
+#define D1_CLOCKS_START() unsigned long long d1c[D1C_N] = {}; long long d1Last = clock64()
+#define D1_TICK(ph) do { const long long now_ = clock64(); d1c[ph] += (unsigned long long)(now_ - d1Last); d1Last = now_; } while (0)
+#define D1_CLOCKS_FLUSH(kernel) do { for (int p_ = 0; p_ < D1C_N; p_++) atomicAdd(&d1_clocks[(kernel) * D1C_N + p_], d1c[p_]); } while (0)
+#else
+#define D1_CLOCKS_START() do { } while (0)
+#define D1_TICK(ph) do { } while (0)
+#define D1_CLOCKS_FLUSH(kernel) do { } while (0)
+#endif
+
 #define SEQ_PACK(ob, ll, ml) ((uint64_t)(ob) | ((uint64_t)(ll) << 30) | ((uint64_t)((ml) - 3u) << 47))
 
 typedef uint16_t SeqEnt;                            // one state of a sequence decoding table (B2Z_SEQ_TAB layout above)
@@ -566,10 +620,12 @@ zstd_dec_lit_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
                             uint8_t* __restrict__ lits, const uint16_t* __restrict__ hufTabs, const LitJob* __restrict__ litJobs) {
     B2Z_EXTERN_SMEM(uint16_t, smTab);                                   // [B2Z_LIT_BLOCKS][2048] decoding tables
     __shared__ uint8_t smW[B2Z_LIT_BLOCKS][256];                        // their weights
+    __shared__ uint64_t smRing[B2Z_LIT_BLOCKS * 4u][B2Z_BWD_DEPTH];     // each thread's FastBwd words in flight
     const uint32_t j = threadIdx.x >> 2, k = threadIdx.x & 3u, bi = blockIdx.x * B2Z_LIT_BLOCKS + j;
     const uint32_t lead = (threadIdx.x & 31u) & ~3u;                    // lane of the block's thread 0
     uint16_t* tab = smTab + (size_t)j * 2048u;
     Src S; S.w = reinterpret_cast<const uint64_t*>(src); S.nWords = (srcSize + 7) >> 3; S.size = srcSize;
+    D1_CLOCKS_START();
     LitJob lj; lj.off = 0; lj.size = 0; lj.regen = 0; lj.streams = 0; lj.type = 0;
     if (bi < nBlocks && blocks[bi].type == 2) lj = litJobs[bi];         // (raw / RLE blocks have no job record)
     // ---- the table: weights (thread 0 of the block), then the fill (the block's 4 threads)
@@ -586,6 +642,7 @@ zstd_dec_lit_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
     __syncwarp();                                                       // the weights are visible to the block's threads
     if (lj.streams && !err) huf_fill(tab, smW[j], nw, maxBits, k, 4u);
     __syncwarp();                                                       // the table is complete
+    D1_TICK(D1C_TABLE);
     if (!lj.streams) return;
     if (err) { if (k == 0) atomicOr(&blocks[bi].status, err); return; }
     // ---- the streams: one thread each
@@ -614,36 +671,39 @@ zstd_dec_lit_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
     }
     if (ok) {
         FastBwd b;
-        if (b.init(&S, off, size)) ok = false;
+        if (b.init(&S, smRing[threadIdx.x], off, size)) ok = false;
         else {
             const uint32_t mb = maxBits;
-            // symbols are gathered eight at a time and stored as one aligned word (head and tail byte by byte): every thread writes its own stream
+            // symbols are gathered eight at a time and stored as one aligned word (head and tail byte by byte): every thread writes its own stream.
+            // Inside a word the reloads come before symbols 0 and 4 in every lane: four symbols of <= 11 bits fit the 57 a reload leaves.
             uint32_t i = 0;
             const uint32_t head = (uint32_t)((8u - ((uintptr_t)dst & 7u)) & 7u);
             for (; i < cnt && i < head; i++) {
-                if (b.consumed > 64u - 11u) b.reload();
+                if (b.consumed > 64u - 11u) { D1_TICK(D1C_DECODE); b.reload(); D1_TICK(D1C_REFILL); }
                 const uint32_t e = tab[(uint32_t)((b.cont << b.consumed) >> (64u - mb))];
-                dst[i] = (uint8_t)e; b.consumed += (e >> 8);
+                D1_TICK(D1C_DECODE); dst[i] = (uint8_t)e; b.consumed += (e >> 8); D1_TICK(D1C_STORE);
             }
             for (; i + 8u <= cnt; i += 8u) {
                 uint64_t acc = 0;
 #pragma unroll
                 for (uint32_t q = 0; q < 8u; q++) {
-                    if (b.consumed > 64u - 11u) b.reload();
+                    if ((q & 3u) == 0) { D1_TICK(D1C_DECODE); b.reload(); D1_TICK(D1C_REFILL); }
                     const uint32_t e = tab[(uint32_t)((b.cont << b.consumed) >> (64u - mb))];
                     acc |= (uint64_t)(e & 255u) << (8u * q); b.consumed += (e >> 8);
                 }
-                *reinterpret_cast<uint64_t*>(dst + i) = acc;
+                D1_TICK(D1C_DECODE); *reinterpret_cast<uint64_t*>(dst + i) = acc; D1_TICK(D1C_STORE);
             }
             for (; i < cnt; i++) {
-                if (b.consumed > 64u - 11u) b.reload();
+                if (b.consumed > 64u - 11u) { D1_TICK(D1C_DECODE); b.reload(); D1_TICK(D1C_REFILL); }
                 const uint32_t e = tab[(uint32_t)((b.cont << b.consumed) >> (64u - mb))];
-                dst[i] = (uint8_t)e; b.consumed += (e >> 8);
+                D1_TICK(D1C_DECODE); dst[i] = (uint8_t)e; b.consumed += (e >> 8); D1_TICK(D1C_STORE);
             }
             ok = b.left() == 0;
+            b.drain();
         }
     }
     if (!ok) atomicOr(&blocks[bi].status, B2Z_DERR_CORRUPT);
+    D1_CLOCKS_FLUSH(0);
 }
 
 // Sequence streams: groups of B2Z_SEQ_BLOCKS blocks, one thread per block (the CTA's other threads leave).  The thread builds its
@@ -656,11 +716,13 @@ zstd_dec_seq_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
                             uint64_t* __restrict__ seqs, const SeqEnt* __restrict__ seqTabs, const SeqJob* __restrict__ seqJobs) {
     __shared__ uint32_t k_seqSym[89];                                   // LL symbols [0,36) | ML symbols [36,89): baseline | extra bits << 24
     __shared__ SeqEnt smTab[B2Z_SEQ_BLOCKS][B2Z_SEQ_TAB];
+    __shared__ uint64_t smRing[B2Z_SEQ_BLOCKS][B2Z_BWD_DEPTH];         // each thread's FastBwd words in flight
     for (uint32_t i = threadIdx.x; i < 89u; i += blockDim.x) k_seqSym[i] = i < 36u ? k_LL_base[i] | ((uint32_t)k_LL_bits[i] << 24) : k_ML_base[i - 36u] | ((uint32_t)k_ML_bits[i - 36u] << 24);
     __syncthreads();
     if (threadIdx.x >= B2Z_SEQ_BLOCKS) return;
     SeqEnt* tab = smTab[threadIdx.x];
     Src S; S.w = reinterpret_cast<const uint64_t*>(src); S.nWords = (srcSize + 7) >> 3; S.size = srcSize;
+    D1_CLOCKS_START();
     for (uint32_t g = blockIdx.x; (uint64_t)g * B2Z_SEQ_BLOCKS < nBlocks; g += gridDim.x) {
         const uint32_t bi = g * B2Z_SEQ_BLOCKS + threadIdx.x;
         if (bi >= nBlocks) break;
@@ -687,9 +749,10 @@ zstd_dec_seq_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
                 }
             }
         }
+        D1_TICK(D1C_TABLE);
         uint32_t regen = 0;
         FastBwd b;
-        if (err || b.init(&S, j.bsOff, j.bsLeft)) err = B2Z_DERR_CORRUPT;
+        if (err || b.init(&S, smRing[threadIdx.x], j.bsOff, j.bsLeft)) err = B2Z_DERR_CORRUPT;
         else {
             const SeqEnt* tL = tab; const SeqEnt* tO = tab + 512; const SeqEnt* tM = tab + 768;
             const uint32_t gL = logs[0], gO = logs[1], gM = logs[2];
@@ -706,20 +769,20 @@ zstd_dec_seq_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
                 if (aO > 30u) { err = B2Z_DERR_UNSUPPORTED; break; }
                 const uint32_t xL = k_seqSym[eL & 63u], xM = k_seqSym[36u + (eM & 63u)];
                 const uint32_t aL = xL >> 24, aM = xM >> 24;
-                b.reload();
+                D1_TICK(D1C_DECODE); b.reload(); D1_TICK(D1C_REFILL);
                 const uint32_t ob = (1u << aO) + b.read(aO);
-                if (aO + aM + aL > 56u) b.reload();
+                if (aO + aM + aL > 56u) { D1_TICK(D1C_DECODE); b.reload(); D1_TICK(D1C_REFILL); }
                 const uint32_t ml = (xM & 0xFFFFFFu) + b.read(aM);
                 const uint32_t ll = (xL & 0xFFFFFFu) + b.read(aL);
                 if (i + 1 < j.nbSeq) {
-                    if (aO + aM + aL > 30u) b.reload();                                                 // + <= 26 state bits
+                    if (aO + aM + aL > 30u) { D1_TICK(D1C_DECODE); b.reload(); D1_TICK(D1C_REFILL); }                                                 // + <= 26 state bits
                     const uint32_t nL = eL >> 6, nM = eM >> 6, nO = eO >> 6;
                     const uint32_t bL = gL - highbit32(nL), bM = gM - highbit32(nM), bO = gO - highbit32(nO);
                     sL = ((nL << bL) - (1u << gL)) + b.read(bL); sM = ((nM << bM) - (1u << gM)) + b.read(bM); sO = ((nO << bO) - (1u << gO)) + b.read(bO);
                 }
                 litUsed += ll; total += ll + ml;
                 if (b.left() < 0 || litUsed > j.litRegen || total > 131072u || ob >= (1u << 30)) { err = B2Z_DERR_CORRUPT; break; }
-                out[i] = SEQ_PACK(ob, ll, ml);
+                D1_TICK(D1C_DECODE); out[i] = SEQ_PACK(ob, ll, ml); D1_TICK(D1C_STORE);
                 // a source at most one unit's span before the block: the block's unit cannot run beside the unit before it (stage D2 counts these)
                 near |= (uint32_t)(ob > 3u && ob - 3u > total - ml && ob - 3u - (total - ml) <= B2Z_DEC_UNIT_BLOCKS * 131072u);
                 if (ob > 3u) { v2 = v1; y2 = y1; v1 = v0; y1 = y0; v0 = ob - 3u; y0 = 0u; }
@@ -733,12 +796,16 @@ zstd_dec_seq_streams_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, D
             blocks[bi].repX[0] = v0; blocks[bi].repX[1] = v1; blocks[bi].repX[2] = v2; blocks[bi].repSym = y0 | (y1 << 2) | (y2 << 4);
             blocks[bi].nearBehind = near;
             if (!err && b.left() != 0) err = B2Z_DERR_CORRUPT;
+            b.drain();
             regen = total + (j.litRegen - litUsed);
             if (regen > 131072u) err = B2Z_DERR_CORRUPT;
         }
+        D1_TICK(D1C_DECODE);
         blocks[bi].regen = err ? 0u : regen; blocks[bi].nbSeq = err ? 0u : j.nbSeq;
         if (err) atomicOr(&blocks[bi].status, err);
+        D1_TICK(D1C_STORE);
     }
+    D1_CLOCKS_FLUSH(1);
 }
 
 // ---------------------------------------------------------------- D2: layout
@@ -1214,6 +1281,15 @@ void launch_zstd_dec_entropy(const uint8_t* src, uint64_t srcSize, DecBlock* blo
       zstd_dec_seq_streams_kernel<<<(nBlocks + B2Z_SEQ_BLOCKS - 1u) / B2Z_SEQ_BLOCKS, 32, 0, st>>>(src, srcSize, blocks, nBlocks, seqs, nullptr, seqJobs); }   // one warp: B2Z_SEQ_BLOCKS chains
     if (stLit != st) { cudaEventRecord(evJoin, stLit); cudaStreamWaitEvent(st, evJoin, 0); }
 }
+#ifdef B2Z_D1_CLOCKS
+// the per-phase cycle sums of every stream thread since the last call (literal kernel's D1C_* order, then the sequence kernel's); clears them
+extern "C" int b200z_d1_clocks(unsigned long long* out) {
+    static const unsigned long long zero[2 * D1C_N] = {};
+    cudaError_t e = cudaMemcpyFromSymbol(out, d1_clocks, sizeof(d1_clocks));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(d1_clocks, zero, sizeof(d1_clocks));
+    return (int)e;
+}
+#endif
 size_t zstd_dec_entropy_scratch_bytes(uint32_t nBlocks) { return (size_t)nBlocks * (sizeof(LitJob) + sizeof(SeqJob)) + 256u; }
 void launch_zstd_dec_layout(DecFrame* frames, uint32_t nFrames, DecBlock* blocks, uint64_t dstCap, DecCounts* counts, uint64_t* total, uint32_t jumpMode, cudaStream_t st) {
     if (nFrames) zstd_dec_frame_sizes_kernel<<<(nFrames + 127) / 128, 128, 0, st>>>(frames, nFrames, blocks, counts, jumpMode);

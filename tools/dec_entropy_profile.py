@@ -1,20 +1,30 @@
 """Where the zstd decoder's entropy stage (D1) spends its time on the bench workload.
 
-  python tools/dec_entropy_profile.py [--size-mib 4096] [--reps 3] [--out FILE]
+  python tools/dec_entropy_profile.py [--size-mib 4096] [--reps 3] [--lib LIB] [--out FILE]
+  python tools/dec_entropy_profile.py --build-clocks DIR       # (no GPU needed) DIR/libb200z.so built with -DB2Z_D1_CLOCKS
 
 Compresses --size-mib MiB of G2 text with the codec's defaults (what bench.py times), then runs decompress_device: one
 warm-up, --reps timed calls with the codec's stage counters (stat 4 = D1, stat 5 = D2 + D3 + verify), and one more call under
 torch.profiler for the per-kernel totals.  Beside them: the card (nvidia-smi) and the shape of the compressed stream from a
 counting pass over its frames on the host (blocks, literal modes, sequences per block, table logs) -- nothing here comes
-from timing.  Set B200Z_LIB to profile another build of the library.  Prints one JSON object (and writes it to --out).
+from timing.  --lib (or B200Z_LIB) profiles another build of the library.
+
+A library built with -DB2Z_D1_CLOCKS also reports the phase split of the two stream kernels: every stream thread adds its
+clock64() cycles per phase (table build, refills, table look-ups and arithmetic, output stores), and the shares of each
+kernel's sum are printed.  The counters cost registers and instructions, so that build's own times are not D1's times.
+Prints one JSON object (and writes it to --out).
 """
 import argparse
+import ctypes
+import glob
 import json
 import os
 import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+PKG = os.path.join(ROOT, "7-zip-zstd_b200")
+PHASES = ["table", "refill", "decode", "store"]            # D1C_* order in csrc/zstd_dec.cu
 sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 
 
@@ -187,10 +197,28 @@ def stream_shape(buf):
 # ---------------------------------------------------------------- GPU
 def card():
     try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
                               capture_output=True, text=True, timeout=30).stdout.strip()
     except Exception as e:
         return f"nvidia-smi unavailable: {e}"
+
+
+def build_clocks(out_dir):
+    """libb200z.so with -DB2Z_D1_CLOCKS into out_dir (the flags of build.sh)."""
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    flags = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC",
+             "-I" + os.path.join(PKG, "csrc"), "-I" + os.path.join(ROOT, "include"), "-DB2Z_D1_CLOCKS"]
+    os.makedirs(out_dir, exist_ok=True)
+    procs, objs = [], []
+    for f in sorted(glob.glob(os.path.join(PKG, "csrc", "*.cu"))):
+        o = os.path.join(out_dir, os.path.basename(f)[:-3] + ".o")
+        procs.append(subprocess.Popen([nvcc, *flags, "-c", f, "-o", o]))
+        objs.append(o)
+    if any(p.wait() for p in procs):
+        raise SystemExit("--build-clocks: compilation failed")
+    lib = os.path.join(out_dir, "libb200z.so")
+    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", lib, *objs, "-lcudart"])
+    print(lib)
 
 
 def main():
@@ -198,11 +226,20 @@ def main():
     ap.add_argument("--size-mib", type=int, default=4096)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--lib", default=None, help="another build of libb200z.so")
+    ap.add_argument("--build-clocks", metavar="DIR", default=None)
     ap.add_argument("--no-shape", action="store_true", help="skip the host counting pass")
     a = ap.parse_args()
+    if a.build_clocks:
+        build_clocks(a.build_clocks)
+        return
+    if a.lib:
+        os.environ["B200Z_LIB"] = os.path.abspath(a.lib)
     import torch
     import __graft_entry__ as ge
     pkg = ge.load_package()
+    clocks = getattr(ctypes.CDLL(pkg.lib_path()), "b200z_d1_clocks", None)
+    buf = (ctypes.c_ulonglong * (2 * len(PHASES)))()
     n = a.size_mib << 20
     host = torch.empty(n, dtype=torch.uint8).pin_memory()
     pkg.corpus.g2_into(host.data_ptr(), n, threads=os.cpu_count() or 8)
@@ -214,12 +251,19 @@ def main():
     assert c.decompress_device(d_comp.data_ptr(), m, d_back.data_ptr(), n) == n          # warm-up (scratch allocations)
     torch.cuda.synchronize()
     rec = {"card": card(), "lib": pkg.lib_path(), "size_mib": a.size_mib, "compressed_bytes": m, "reps": []}
+    if clocks:
+        clocks(buf)                                                 # drop the warm-up's counts
     for _ in range(a.reps):
         c.reset_stats(); torch.cuda.synchronize()
         assert c.decompress_device(d_comp.data_ptr(), m, d_back.data_ptr(), n) == n
         torch.cuda.synchronize()
         rec["reps"].append({"dec_prepass_ms": c.stat(9), "dec_entropy_ms": c.stat(4), "dec_exec_ms": c.stat(5)})
     assert torch.equal(d_back, d_in), "round trip mismatch"
+    if clocks:
+        assert clocks(buf) == 0
+        for k, name in enumerate(["zstd_dec_lit_streams_kernel", "zstd_dec_seq_streams_kernel"]):
+            v = buf[k * len(PHASES):(k + 1) * len(PHASES)]; tot = max(1, sum(v))
+            rec.setdefault("phase_share", {})[name] = {p: round(v[i] / tot, 4) for i, p in enumerate(PHASES)}
     from torch.profiler import profile, ProfilerActivity
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         c.decompress_device(d_comp.data_ptr(), m, d_back.data_ptr(), n)
