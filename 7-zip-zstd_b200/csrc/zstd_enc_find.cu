@@ -13,6 +13,13 @@
 // hops per CH positions; the result is the pure function of the frame's bytes that
 // oracle/zstd_enc_oracle.c:b2zo_zstd_candidates states position by position.
 //
+// Per iteration a position hashes its 16 bytes (loaded one iteration ahead), takes the turn, and then requests the next
+// iteration's bytes and both candidates' bytes together, one L2 round trip, before comparing either.  Level 3 (<4, 7, 0>, 896
+// threads): 56 registers, no spills; the GUARD = false loop is 159 SASS instructions per position (199 before, cuobjdump -sass).
+// Stage F per 4 GiB step of the bench: 43.3 -> 35.4 ms on an H100 80GB HBM3 (700 W, 1980 MHz).  The clock split of that build
+// (-DB2Z_F_CLOCKS) puts 70 % of a warp's cycles between the candidates' loads and their lengths, 15 % in the turn and under 2 %
+// waiting for it (DESIGN 2.2).
+//
 // Output: one candidate word per position (B2Z_CAND: offset << 7 | length, 0 = none), consumed by stage G
 // (zstd_enc_dp.cu).  Replaces the finder half of zstd_double_fast.c:103-330 (ZSTD_compressBlock_doubleFast_noDict_generic:
 // hashLong / hashSmall look-ups and inserts, ZSTD_count), the table upkeep of zstd_compress.c:4591 and the job slicing of
@@ -38,54 +45,95 @@ __device__ __forceinline__ void turn_inputs_ready(uint32_t* slot, uint32_t iL, u
 }
 
 // 16 bytes at any byte offset as four 32-bit words: five aligned 32-bit loads and four native funnel shifts (the 64-bit formulation
-// costs eight ALU instructions per 8 bytes; the ALU pipe is this kernel's bound).  GUARD: words at or beyond nW4 read as zero (only
+// costs eight ALU instructions per 8 bytes).  GUARD: words at or beyond nW4 read as zero (only
 // the last frame of a buffer needs it: any other frame is followed by readable bytes, and a length is clipped to the frame anyway).
 struct B16 { uint32_t x0, x1, x2, x3; };
 static_assert(B2Z_CAP == 16, "stage F compares four 32-bit words");
-template <bool GUARD>
-__device__ __forceinline__ B16 ld16(const uint32_t* __restrict__ w4, uint32_t o, uint32_t nW4) {
-    const uint32_t a = o >> 2, sh = (o & 3u) * 8u;
-    uint32_t t0, t1, t2, t3, t4;
-    if (GUARD) {
-        t0 = a < nW4 ? __ldg(w4 + a) : 0u; t1 = a + 1u < nW4 ? __ldg(w4 + a + 1u) : 0u; t2 = a + 2u < nW4 ? __ldg(w4 + a + 2u) : 0u;
-        t3 = a + 3u < nW4 ? __ldg(w4 + a + 3u) : 0u; t4 = a + 4u < nW4 ? __ldg(w4 + a + 4u) : 0u;
-    } else { t0 = __ldg(w4 + a); t1 = __ldg(w4 + a + 1u); t2 = __ldg(w4 + a + 2u); t3 = __ldg(w4 + a + 3u); t4 = __ldg(w4 + a + 4u); }
+// (The funnel shift takes its amount mod 32, so o * 8 is the byte shift.)  ld16p: the words at w, shifted by sh, unguarded.
+__device__ __forceinline__ B16 ld16p(const uint32_t* __restrict__ w, uint32_t sh) {
+    const uint32_t t0 = __ldg(w), t1 = __ldg(w + 1), t2 = __ldg(w + 2), t3 = __ldg(w + 3), t4 = __ldg(w + 4);
     B16 r; r.x0 = __funnelshift_r(t0, t1, sh); r.x1 = __funnelshift_r(t1, t2, sh); r.x2 = __funnelshift_r(t2, t3, sh); r.x3 = __funnelshift_r(t3, t4, sh);
     return r;
 }
-// common-prefix length (0..16) of two 16-byte strings
+template <bool GUARD>
+__device__ __forceinline__ B16 ld16(const uint32_t* __restrict__ w4, uint32_t o, uint32_t nW4) {
+    const uint32_t a = o >> 2, sh = o * 8u;
+    if (!GUARD) return ld16p(w4 + a, sh);
+    const uint32_t t0 = a < nW4 ? __ldg(w4 + a) : 0u, t1 = a + 1u < nW4 ? __ldg(w4 + a + 1u) : 0u, t2 = a + 2u < nW4 ? __ldg(w4 + a + 2u) : 0u;
+    const uint32_t t3 = a + 3u < nW4 ? __ldg(w4 + a + 3u) : 0u, t4 = a + 4u < nW4 ? __ldg(w4 + a + 4u) : 0u;
+    B16 r; r.x0 = __funnelshift_r(t0, t1, sh); r.x1 = __funnelshift_r(t1, t2, sh); r.x2 = __funnelshift_r(t2, t3, sh); r.x3 = __funnelshift_r(t3, t4, sh);
+    return r;
+}
+// common-prefix length (0..15) of two 16-byte strings, or a number above 16 when all 16 bytes agree (__ffs(0) - 1 wraps): the
+// caller clips it to at most 16 anyway
 __device__ __forceinline__ uint32_t prefix16(const B16& a, const B16& b) {
     const uint32_t d0 = a.x0 ^ b.x0, d1 = a.x1 ^ b.x1, d2 = a.x2 ^ b.x2, d3 = a.x3 ^ b.x3;
     const uint32_t z = d0 ? d0 : (d1 ? d1 : (d2 ? d2 : d3));
     const uint32_t base = d0 ? 0u : (d1 ? 4u : (d2 ? 8u : 12u));
-    return z ? base + ((uint32_t)(__ffs((int)z) - 1) >> 3) : 16u;
+    return base + ((uint32_t)(__ffs((int)z) - 1) >> 3);
 }
 
 // MODE 0: both tables (levels 3-4); 1: only the short table (levels 1-2, fast levels); 2: both tables + the lower lanes of a
 // position's own step (levels 5-7) -- b2z_params.h: B2Z_FLAG_FIND_FAST / B2Z_FLAG_FIND_STEP
 struct FindCtx {
-    uint32_t* smem; uint32_t* TL; uint32_t* TS; uint32_t tableWords, HL, HS, tagBits, tagMask, W, tid, grp, tg, nextGrp;
+    uint32_t* smem; uint32_t* TL; uint32_t* TS; uint32_t tableWords, HL, HS, tagBits, tagMask, W, tid, grp, tg;
+    uint32_t barTurn, barGrp, barNext;                                         // named barrier ids of this thread's group
 };
 
+// -DB2Z_F_CLOCKS (off by default; tools/enc_find_profile.py --build-clocks): every warp adds the clock64() cycles it spends in each
+// phase to f_clocks[]; b200z_find_clocks() reads and clears them.  Without the switch the ticks compile to nothing.
+//   wait: bar.sync of the turn (the previous group still holds it); turn: table reads, group barrier, atomics, hand-over;
+//   cand: from the candidates' loads to their compared lengths (mostly the L2 round trip); work: hash, prefetch, pack, store.
+enum { FC_WAIT, FC_TURN, FC_CAND, FC_WORK, FC_N };
+#ifdef B2Z_F_CLOCKS
+__device__ unsigned long long f_clocks[FC_N + 1];                             // [FC_N] = warps
+#define F_TICK(ph) do { const long long now_ = clock64(); fc[ph] += (unsigned long long)(now_ - fcLast); fcLast = now_; } while (0)
+#else
+#define F_TICK(ph) do { } while (0)
+#endif
+
 // the chunks of one frame (n bytes at w4, candidate words to out)
+//
+// Per position and iteration: hash the 16 bytes loaded one iteration ahead, take the turn, request the next iteration's bytes and
+// BOTH candidates' 16 bytes at once (no branch between the loads: a candidate that fails its tag or window test loads the position's
+// own bytes and gets length 0), then compare.  The output pointer and the own bytes' word index advance by a step per iteration;
+// the own bytes' shift is fixed per frame (p mod 4 never changes: a step is G * CH positions).
 template <int WPG, int G, int MODE, bool GUARD>
-__device__ __forceinline__ void find_frame(const FindCtx& c, const uint32_t* __restrict__ w4, uint32_t n, uint32_t* __restrict__ out) {
-    constexpr uint32_t CH = WPG * 32u;
+__device__ __forceinline__ void find_frame(const FindCtx& c, const uint32_t* __restrict__ w4, uint32_t n, uint32_t* __restrict__ out
+#ifdef B2Z_F_CLOCKS
+                                           , unsigned long long* fc, long long& fcLast
+#endif
+                                           ) {
+    constexpr uint32_t CH = WPG * 32u, STEPW = G * CH;
     constexpr bool FAST = MODE == 1, STEP = MODE == 2;
     const uint32_t nW4 = (n + 3u) >> 2;
-    const uint32_t HL = c.HL, HS = c.HS, tagBits = c.tagBits, tagMask = c.tagMask;
+    const uint32_t HL = c.HL, HS = c.HS, tagBits = c.tagBits, W = c.W;
+    uint32_t tagMask = c.tagMask;
+#ifndef B2Z_CUEMU
+    // held in registers for the whole frame: without the opaque moves ptxas recomputes both in the loop (4 + 3 instructions)
+    asm("mov.b64 %0, %0;" : "+l"(w4)); asm("mov.b32 %0, %0;" : "+r"(tagMask));
+#endif
+    // the index and the tag are the top HL + tagBits bits of the 64-bit product, and HL + tagBits <= 15 + (31 - 17) < 32
+    // (launch_zstd_enc_find checks it): only the high word of each product is formed.  (v << 24) * PRIME5 = v * (PRIME5 << 24).
+    constexpr uint64_t PL = B2Z_PRIME8, PS = B2Z_PRIME5 << 24;
+    const uint32_t shIL = 32u - HL, shIS = 32u - HS, shTL = 32u - HL - tagBits, shTS = 32u - HS - tagBits;
     const uint32_t nChunks = (n + CH - 1u) / CH, nIter = (nChunks + G - 1u) / G;
-    B16 vNext = ld16<true>(w4, c.grp * CH + c.tg, nW4);
-    for (uint32_t it = 0; it < nIter; it++) {
-        const uint32_t p = (it * G + c.grp) * CH + c.tg;
+    uint32_t p = c.grp * CH + c.tg;
+    B16 vNext = ld16<true>(w4, p, nW4);
+    uint32_t aNext = (p >> 2) + STEPW / 4u;                               // the next iteration's own first word ...
+    const uint32_t shOwn = p * 8u;                                        // ... and byte shift (p mod 4 = tg mod 4 for the whole frame)
+    uint32_t* __restrict__ o = out + p;
+    for (uint32_t it = 0; it < nIter; it++, p += STEPW, aNext += STEPW / 4u, o += STEPW) {
         // ---- before the turn: the 16 bytes at p (loaded one iteration ahead), hashes, same-step groups
         const B16 own = vNext;
-        const uint64_t v = (uint64_t)own.x0 | ((uint64_t)own.x1 << 32);
         const bool hashable = p + 8u <= n;                                 // p >= n for the padding chunks of the last iteration
-        const uint64_t hl = v * B2Z_PRIME8, hs = (v << 24) * B2Z_PRIME5;
-        const uint32_t iL = (uint32_t)(hl >> (64u - HL)), iS = (uint32_t)(hs >> (64u - HS));
-        const uint32_t tL = (uint32_t)(hl >> (64u - HL - tagBits)) & tagMask, tS = (uint32_t)(hs >> (64u - HS - tagBits)) & tagMask;
+        const uint32_t hl = (uint32_t)(((uint64_t)own.x0 * (uint32_t)PL) >> 32) + own.x0 * (uint32_t)(PL >> 32) + own.x1 * (uint32_t)PL;
+        const uint32_t hs = (uint32_t)(((uint64_t)own.x0 * (uint32_t)PS) >> 32) + own.x0 * (uint32_t)(PS >> 32) + own.x1 * (uint32_t)PS;
+        const uint32_t iL = hl >> shIL, iS = hs >> shIS;
+        const uint32_t tL = (hl >> shTL) & tagMask, tS = (hs >> shTS) & tagMask;
         const uint32_t mineL = ((p + 1u) << tagBits) | tL, mineS = ((p + 1u) << tagBits) | tS;
+        // what the turn writes: max with 0 leaves an entry as it is, so a padding position's atomics need no branch
+        const uint32_t putL = hashable ? mineL : 0u, putS = hashable ? mineS : 0u;
         uint32_t* const aL = c.TL + iL; uint32_t* const aS = c.TS + iS;
         uint32_t lowL = 0, lowS = 0;
         if (STEP) {                                                        // lanes of this step with my table index, below me
@@ -93,35 +141,49 @@ __device__ __forceinline__ void find_frame(const FindCtx& c, const uint32_t* __r
             lowL = __match_any_sync(B2Z_FULL, hashable ? iL : (0x80000000u | lane)) & lt;
             lowS = __match_any_sync(B2Z_FULL, hashable ? iS : (0x80000000u | lane)) & lt;
         }
-        turn_inputs_ready(c.smem + c.tableWords + c.tid, iL, iS, mineL, mineS, (uint32_t)hashable ^ lowL ^ (lowS << 1));
+        turn_inputs_ready(c.smem + c.tableWords + c.tid, iL, iS, putL, putS, c.barNext ^ lowL ^ (lowS << 1));
+        F_TICK(FC_WORK);
         // ---- the turn: nothing but the table accesses between the two barrier hops
-        bar_sync(B2Z_FIND_BAR_TURN(c.grp), 2u * CH);
-        uint32_t eL = 0, eS = 0;
-        if (hashable) { if (!FAST) eL = *aL; eS = *aS; }
-        if (WPG > 1) bar_sync(B2Z_FIND_BAR_GRP(c.grp), CH); else __syncwarp();
-        if (hashable) { if (!FAST) atomicMax(aL, mineL); atomicMax(aS, mineS); }     // the highest position of the chunk stays
-        bar_arrive(B2Z_FIND_BAR_TURN(c.nextGrp), 2u * CH);
+        bar_sync(c.barTurn, 2u * CH);
+        F_TICK(FC_WAIT);
+        uint32_t eL = 0, eS;
+        if (!FAST) eL = *aL;
+        eS = *aS;
+        if (WPG > 1) bar_sync(c.barGrp, CH); else __syncwarp();
+        if (!FAST) atomicMax(aL, putL);                                    // the highest position of the chunk stays
+        atomicMax(aS, putS);
+        bar_arrive(c.barNext, 2u * CH);
+        F_TICK(FC_TURN);
         if (STEP) {                                                        // a lower lane of the step with my index is nearer than the table's entry
             const uint32_t fromL = __shfl_sync(B2Z_FULL, mineL, lowL ? 31 - __clz((int)lowL) : 0);
             const uint32_t fromS = __shfl_sync(B2Z_FULL, mineS, lowS ? 31 - __clz((int)lowS) : 0);
             if (lowL) eL = fromL;
             if (lowS) eS = fromS;
         }
-        // ---- after the turn: the next iteration's bytes are requested before this one's candidates are compared
-        vNext = ld16<GUARD>(w4, p + G * CH, nW4);
+        // ---- after the turn: the next iteration's bytes and both candidates are requested before either is compared
+        if (GUARD) vNext = ld16<true>(w4, p + STEPW, nW4);
+        else vNext = ld16p(w4 + aNext, shOwn);
         uint32_t word = 0;
-        if (hashable) {
+        if (hashable) {                                                    // (the branch also keeps ptxas from hoisting the loads into the turn)
+            const uint32_t offL = p - ((eL >> tagBits) - 1u), offS = p - ((eS >> tagBits) - 1u);
+            const bool okL = !FAST && hashable && eL && (eL & tagMask) == tL && offL <= W;
+            const bool okS = hashable && eS && (eS & tagMask) == tS && offS <= W && !(okL && offS == offL);   // not the long one's offset
+            const B16 cL = ld16<GUARD>(w4, p - (okL ? offL : 0u), nW4);
+            const B16 cS = ld16<GUARD>(w4, p - (okS ? offS : 0u), nW4);
             // at most B2Z_CAP = 16 bytes are compared, never beyond the position's 4 KiB parse segment
             const uint32_t segEnd = ((p | (B2Z_SEG - 1u)) + 1u) < n ? ((p | (B2Z_SEG - 1u)) + 1u) : n;
             const uint32_t maxLen = (segEnd - p) < B2Z_CAP ? (segEnd - p) : B2Z_CAP;
-            uint32_t lenL = 0, offL = 0, lenS = 0, offS = 0;
-            if (eL && (eL & tagMask) == tL) { const uint32_t q = (eL >> tagBits) - 1u; if (p - q <= c.W) { offL = p - q; const uint32_t l = prefix16(ld16<GUARD>(w4, q, nW4), own); lenL = l < maxLen ? l : maxLen; } }
-            if (eS && (eS & tagMask) == tS) { const uint32_t q = (eS >> tagBits) - 1u; if (p - q <= c.W && p - q != offL) { offS = p - q; const uint32_t l = prefix16(ld16<GUARD>(w4, q, nW4), own); lenS = l < maxLen ? l : maxLen; } }
-            uint32_t len = lenL, off = offL;
-            if (lenS > lenL || (lenS == lenL && lenS && offS < offL)) { len = lenS; off = offS; }
-            if (len >= B2Z_DP_MINLEN) word = B2Z_CAND(len, off);
+            const uint32_t lL = prefix16(cL, own), lS = prefix16(cS, own);
+            F_TICK(FC_CAND);
+            const uint32_t mL = okL ? maxLen : 0u, mS = okS ? maxLen : 0u;
+            const uint32_t lenL = FAST ? 0u : (lL < mL ? lL : mL), lenS = lS < mS ? lS : mS;
+            // the longer wins, the nearer of two equally long ones (offsets < 2^24: a frame is at most 2^B2Z_MAX_FRAMELOG bytes); a
+            // length below B2Z_DP_MINLEN makes the word 0 whichever side it came from
+            const uint32_t kL = (lenL << 24) | (~offL & 0xFFFFFFu), kS = (lenS << 24) | (~offS & 0xFFFFFFu);
+            const uint32_t k = kS > kL ? kS : kL, len = k >> 24;
+            word = len >= B2Z_DP_MINLEN ? B2Z_CAND(len, ~k & 0xFFFFFFu) : 0u;
         }
-        if (p < n) __stcs(out + p, word);                                  // streaming: the words are next read by another kernel
+        if (p < n) __stcs(o, word);                                        // streaming: the words are next read by another kernel
     }
 }
 
@@ -141,9 +203,17 @@ zstd_enc_find_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom 
     c.tableWords = (MODE == 1 ? 0u : (1u << c.HL)) + (1u << c.HS);
     c.tagBits = 32u - (g.frameLog + 1u); c.tagMask = (1u << c.tagBits) - 1u;
     c.W = g.windowLog >= 32 ? 0xFFFFFFFFu : (1u << g.windowLog);
-    c.nextGrp = c.grp + 1u == (uint32_t)G ? 0u : c.grp + 1u;
+    c.barTurn = B2Z_FIND_BAR_TURN(c.grp); c.barGrp = B2Z_FIND_BAR_GRP(c.grp);
+    c.barNext = B2Z_FIND_BAR_TURN(c.grp + 1u == (uint32_t)G ? 0u : c.grp + 1u);
     const uint64_t nFrames = (srcSize + (1ull << g.frameLog) - 1) >> g.frameLog;
     const uint32_t tid = c.tid;
+#ifdef B2Z_F_CLOCKS
+    unsigned long long fc[FC_N] = {};
+    long long fcLast = clock64();
+#define B2Z_F_CLOCK_ARGS , fc, fcLast
+#else
+#define B2Z_F_CLOCK_ARGS
+#endif
 
     // the first turn of the kernel belongs to group 0 and nobody hands it over: the last group arrives once up front.
     // Afterwards every frame runs a multiple of G chunks, so the hand-over that closes a frame opens the next one.
@@ -166,13 +236,18 @@ zstd_enc_find_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom 
         __syncthreads();                                                       // flag seen; previous frame's table accesses done
         for (uint32_t i = tid; i < c.tableWords / 4u; i += NT) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
         __syncthreads();
+        F_TICK(FC_WORK);
         // a frame followed by at least 4 KiB of the buffer needs no bounds checks on its loads (they reach at most 2 * 896 + 20 bytes
         // past the frame: the prefetch of a padding chunk)
-        if (srcSize - f0 - n >= 4096u) find_frame<WPG, G, MODE, false>(c, w4, n, out);
-        else find_frame<WPG, G, MODE, true>(c, w4, n, out);
+        if (srcSize - f0 - n >= 4096u) find_frame<WPG, G, MODE, false>(c, w4, n, out B2Z_F_CLOCK_ARGS);
+        else find_frame<WPG, G, MODE, true>(c, w4, n, out B2Z_F_CLOCK_ARGS);
     }
+#undef B2Z_F_CLOCK_ARGS
     // leave the barriers balanced: the hand-over that closed the last frame is consumed by group 0
     if (c.grp == 0) bar_sync(B2Z_FIND_BAR_TURN(0), 2u * CH);
+#ifdef B2Z_F_CLOCKS
+    if ((tid & 31u) == 0) { for (int p_ = 0; p_ < FC_N; p_++) atomicAdd(&f_clocks[p_], fc[p_]); atomicAdd(&f_clocks[FC_N], 1ull); }
+#endif
 }
 
 #ifndef B2Z_CUEMU
@@ -200,6 +275,9 @@ static cudaError_t launch_find_t(const uint8_t* src, uint64_t srcSize, const Enc
 cudaError_t launch_zstd_enc_find(const uint8_t* src, uint64_t srcSize, const EncGeom& g, uint32_t* cand, uint32_t nCtas,
                                  const uint32_t* ready, uint32_t readyShift, uint32_t* errFlag, cudaStream_t st) {
     if (srcSize == 0) return cudaSuccess;
+    // find_frame hashes with the high words of the products only, and packs an offset into 24 bits
+    const uint32_t hashLog = g.hashLogL > g.hashLogS ? g.hashLogL : g.hashLogS;
+    if (g.frameLog < 17 || g.frameLog > B2Z_MAX_FRAMELOG || hashLog + 31u - g.frameLog > 32u) return cudaErrorInvalidValue;
     switch (g.chunkLog) {
     case 5: return launch_find_t<1, 7>(src, srcSize, g, cand, nCtas, ready, readyShift, errFlag, st);
     case 6: return launch_find_t<2, 7>(src, srcSize, g, cand, nCtas, ready, readyShift, errFlag, st);
@@ -208,6 +286,16 @@ cudaError_t launch_zstd_enc_find(const uint8_t* src, uint64_t srcSize, const Enc
     }
     return cudaErrorInvalidValue;
 }
+
+#ifdef B2Z_F_CLOCKS
+// the per-phase cycle sums of every warp since the last call (FC_* order, then the warp count); clears them
+extern "C" int b200z_find_clocks(unsigned long long* out) {
+    static const unsigned long long zero[FC_N + 1] = {};
+    cudaError_t e = cudaMemcpyFromSymbol(out, f_clocks, sizeof(f_clocks));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(f_clocks, zero, sizeof(f_clocks));
+    return (int)e;
+}
+#endif
 #endif
 
 }  // namespace b2z
