@@ -9,13 +9,15 @@
 //      next B2Z_CAP costs are live (candidates are at most B2Z_CAP long), kept in a per-lane ring in shared memory, cost[i+1]
 //      also in a register, and the match price is formed four positions ahead of the chain (dp_match); the choice (0 = literal,
 //      else the length) goes to a byte array in HBM, four positions per store;
-//   3. per lane, a forward walk that only counts (sequences, literals, where the last match ends) -- a chosen match of
-//      the full B2Z_CAP bytes is extended by direct comparison to the segment end;
+//   3. per lane, one forward walk over the path: a chosen match of the full B2Z_CAP bytes is extended by direct comparison
+//      to the segment end, each match becomes its (offBase, litLength, matchLength) record, staged at the lane's own run of
+//      the block's sequence array, and each tile's path literals become a 32-bit mask, kept where the tile's choices were.
+//      The repcode history is "unknown" at every segment start, so no lane waits for another; only the first record's
+//      literal length depends on the lanes before;
 //   4. warp scans turn the counts into each lane's place in the block's sequence and literal arrays and into the literal
 //      run that reaches into a lane from the lanes before it;
-//   5. the same walk again, emitting final (offBase, litLength, matchLength) records and the literal bytes (a tile's literals
-//      one lane's run per store, dp_emit_literals).  The repcode
-//      history is "unknown" at every segment start, so no lane waits for another.
+//   5. the move packs the staged records behind each other and completes each lane's first literal length;
+//   6. the literal bytes, from the source tiles and the masks (a tile's literals one lane's run per store, dp_emit_literals).
 // A block of one repeated byte becomes the single sequence that stage E stores as an RLE block.
 //
 // Role in the reference: the parse half of ZSTD_compressBlock_doubleFast_noDict_generic (zstd_double_fast.c:103-330: which
@@ -33,17 +35,29 @@ namespace b2z {
 // choices) coalesced pieces, read by lane j along its padded row (stride 33 / 9 words: conflict-free).
 constexpr uint32_t DP_RING = 32;
 static_assert(DP_RING > B2Z_CAP && (DP_RING & (DP_RING - 1u)) == 0, "the ring holds cost[i + 1 .. i + B2Z_CAP] while cost[i] is written");
+// The walk stages lane j's records at out + DP_LANE_SEQS * j (a match is at least B2Z_DP_MINLEN long), and the move packs them
+// behind each other once the warp scan has placed every lane.
+constexpr uint32_t DP_LANE_SEQS = B2Z_SEG / B2Z_DP_MINLEN;
+static_assert(32u * DP_LANE_SEQS <= B2Z_MAXSEQ, "every lane's records fit its staging run in the block's sequence array");
+// records a lane keeps in shared memory between stores: at most 8 start in one tile (32 positions / B2Z_DP_MINLEN), and the warp stores
+// them once a lane holds more than 8
+constexpr uint32_t DP_PEND = 16;
+static_assert(32u / B2Z_DP_MINLEN <= DP_PEND / 2u, "a tile's records fit behind the ones a lane may still hold");
 struct DpWarpSmem {
-    uint32_t ring[DP_RING][32];  // cost ring: [position & (DP_RING - 1)][lane]; a candidate reaches at most B2Z_CAP positions ahead
+    union {
+        uint32_t ring[DP_RING][32];  // programme: cost ring [position & (DP_RING - 1)][lane]; a candidate reaches at most B2Z_CAP positions ahead
+        uint64_t recs[32][DP_PEND];  // walk: [lane][record ^ (lane & 15)] (the swizzle keeps the walk's writes and the stores' reads conflict-free)
+        uint32_t runs[3][33];        // move: per lane its first record's place, the distance back from its staging run, its literal-length patch
+    };
     uint32_t candTile[32][33];   // [lane][position in tile]; the byte histogram (256 words) lives here before the first tile
-    uint32_t srcTile[32][9];     // [lane][4 input bytes]
-    uint32_t chcTile[32][9];     // [lane][4 choices]
+    uint32_t srcTile[32][9];     // [lane][4 input bytes]; the walk keeps the path-literal masks of up to 8 tiles here
+    uint32_t chcTile[32][9];     // [lane][4 choices]; the literal pass reads the masks back into it
     uint8_t litc[256];
 };
 
 // -DB2Z_DP_CLOCKS (off by default; tools/enc_parse_profile.py --build-clocks): every warp adds the clock64() cycles it spends in each
 // phase to dp_clocks[]; b200z_dp_clocks() reads and clears them.  Without the switch the ticks compile to nothing.
-enum { DPC_HIST, DPC_DP_LOAD, DPC_DP, DPC_DP_STORE, DPC_CNT_LOAD, DPC_CNT, DPC_SCAN, DPC_EMIT_LOAD, DPC_EMIT, DPC_N };
+enum { DPC_HIST, DPC_DP_LOAD, DPC_DP, DPC_DP_STORE, DPC_WALK_LOAD, DPC_WALK, DPC_WALK_STORE, DPC_SCAN, DPC_MOVE, DPC_LIT_LOAD, DPC_LIT, DPC_N };
 #ifdef B2Z_DP_CLOCKS
 __device__ unsigned long long dp_clocks[DPC_N + 1];                         // [DPC_N] = warps
 #define DP_TICK(ph) do { const long long now_ = clock64(); dpc[ph] += (unsigned long long)(now_ - dpLast); dpLast = now_; } while (0)
@@ -65,9 +79,8 @@ __device__ __forceinline__ uint32_t dp_log16(uint32_t x) {
 
 // Tiles are fetched into registers one tile ahead of the pass that uses them (fetch t+1 -- or t-1 in the backward DP -- right after
 // putting tile t into shared memory), so a tile's loads are in flight while the warp works on the one before: r[j] = row j's word in
-// column `lane`.  40 (DP pass) to 48 (emit pass) registers per lane: 128 in all, 4 CTAs = 16 warps per SM, which measured faster
-// than the 20 warps of a 96-register build that fetched the emit pass's candidate tile without the look-ahead.  A second set of
-// shared-memory tiles would cost 5.4 KB per warp.
+// column `lane`: 40 registers per lane in the DP pass and the walk, 16 in the literal pass.  A second set of shared-memory tiles
+// would cost 5.4 KB per warp.
 // tile t of a 32-bit-per-position array: 32 coalesced 128-byte rows, all issued at once.  base = the block's array, bn = positions in the block
 __device__ __forceinline__ void dp_fetch_cand(uint32_t (&r)[32], const uint32_t* __restrict__ base, uint32_t bn, uint32_t t, uint32_t lane) {
 #pragma unroll
@@ -80,12 +93,15 @@ __device__ __forceinline__ void dp_put_cand(DpWarpSmem& sm, const uint32_t (&r)[
 #pragma unroll
     for (uint32_t j = 0; j < 32u; j++) sm.candTile[j][lane] = r[j];
 }
-// tile t of a byte-per-position array: 8 loads of 4 rows x 32 bytes
+// tile t of a byte-per-position array: 8 loads of 4 rows x 32 bytes.  WRITTEN: the words were stored earlier in this kernel (the
+// path-literal masks), so they are read through L2 (__ldcg) and not through the non-coherent cache
+template <bool WRITTEN = false>
 __device__ __forceinline__ void dp_fetch_bytes(uint32_t (&r)[8], const uint8_t* __restrict__ base, uint32_t bn, uint32_t t, uint32_t lane) {
 #pragma unroll
     for (uint32_t k = 0; k < 8u; k++) {
         const uint32_t row = 4u * k + (lane >> 3), wd = lane & 7u, pos = row * B2Z_SEG + 32u * t + 4u * wd;
-        r[k] = pos < bn ? __ldg(reinterpret_cast<const uint32_t*>(base + pos)) : 0u;
+        const uint32_t* const p = reinterpret_cast<const uint32_t*>(base + pos);
+        r[k] = pos < bn ? (WRITTEN ? __ldcg(p) : __ldg(p)) : 0u;
     }
 }
 __device__ __forceinline__ void dp_put_bytes(uint32_t (*tile)[9], const uint32_t (&r)[8], uint32_t lane) {
@@ -120,10 +136,10 @@ __device__ __forceinline__ void dp_match(const DpWarpSmem& sm, uint32_t lane, ui
     mh = p >= lim ? 0u : len - (m & 3u);
 }
 
-// per-lane state of the forward walk over a segment's choices
+// per-lane state of the forward walk over a segment's choices (positions segment-relative)
 struct DpWalk {
-    uint32_t i, ns, nl, lastEnd;            // segment-relative position; sequences / literals so far; block-relative end of the last match
-    uint32_t rep0, rep1, rep2, prevEnd;     // EMIT only
+    uint32_t i, ns, nl, np;                 // position; sequences / literals so far; records not yet stored
+    uint32_t prevEnd, rep0, rep1, rep2;     // end of the last match (0 before the first); repcode history
 };
 
 // bit t of the result: byte t of the lane's 32-byte row is not zero (4 bytes per step: carry-free "byte != 0", then a multiply that
@@ -141,13 +157,13 @@ __device__ __forceinline__ uint32_t dp_nonzero_mask(const uint32_t* row) {
 
 // one tile of the forward walk: positions [32 t, 32 t + 32) of the lane's segment, as far as the lane's path touches them.  On the
 // path, literals are exactly the positions up to the next non-zero choice, so a whole literal run is one iteration (find-first-set on
-// the tile's "choice != 0" mask), and the loop runs once per match instead of once per position.  EMIT: returns the tile's positions
-// that are literals of the path (bit w = position 32 t + w), which dp_emit_literals writes out.
-template <bool EMIT>
-__device__ __forceinline__ uint32_t dp_walk_tile(DpWarpSmem& sm, DpWalk& k, uint32_t t, uint32_t lane, uint32_t sn, uint32_t s0 /* block-relative */,
-                                             const uint64_t* __restrict__ fw /* frame as words */, uint32_t segAbs /* frame-relative */, uint32_t nWords,
-                                             const uint32_t* __restrict__ cnd /* segment's candidate words */,
-                                             uint64_t* __restrict__ outSeq) {
+// the tile's "choice != 0" mask), and the loop runs once per match instead of once per position.  Each match becomes its final
+// (offBase, litLength, matchLength) record in sm.recs, except that the segment's first record counts its literals from the segment
+// start: the repcode history is "unknown" (0) there, so that record is coded with its explicit offset whatever the lanes before
+// left, and only its literal length waits for the warp scan.  Returns the tile's positions that are literals of the path (bit w =
+// position 32 t + w), which dp_emit_literals writes out after the scan.
+__device__ __forceinline__ uint32_t dp_walk_tile(DpWarpSmem& sm, DpWalk& k, uint32_t t, uint32_t lane, uint32_t sn,
+                                                 const uint64_t* __restrict__ fw /* frame as words */, uint32_t segAbs /* frame-relative */, uint32_t nWords) {
     const uint32_t tEnd = (32u * t + 32u) < sn ? (32u * t + 32u) : sn;
     uint32_t lits = 0;
     if (k.i >= tEnd) return lits;
@@ -158,37 +174,45 @@ __device__ __forceinline__ uint32_t dp_walk_tile(DpWarpSmem& sm, DpWalk& k, uint
         const uint32_t rem = M >> w;
         const uint32_t r = rem ? (uint32_t)(__ffs((int)rem) - 1) : (tEnd - k.i);        // literals up to the next match of the tile (or the tile's end)
         if (r) {
-            if (EMIT) lits |= (0xFFFFFFFFu >> (32u - r)) << w;
+            lits |= (0xFFFFFFFFu >> (32u - r)) << w;
             k.nl += r; k.i += r; w += r;
             if (!rem) break;
         }
         uint32_t l = (sm.chcTile[lane][w >> 2] >> (8u * (w & 3u))) & 255u;
-        const uint32_t off = EMIT ? B2Z_CAND_OFF(sm.candTile[lane][w]) : 0u;
-        if (l == B2Z_CAP) {                                                    // the full common prefix, to the segment end at most
-            const uint32_t o = EMIT ? off : B2Z_CAND_OFF(__ldg(cnd + k.i));
-            l = match_len(fw, segAbs + k.i - o, segAbs + k.i, sn - k.i, nWords);
-        }
-        if (EMIT) {
-            const uint32_t pos = s0 + k.i, ll = pos - k.prevEnd;
-            uint32_t code = 0, offBase;
-            if (ll) { if (off == k.rep0) code = 1; else if (off == k.rep1) code = 2; else if (off == k.rep2) code = 3; }
-            else { if (off == k.rep1) code = 1; else if (off == k.rep2) code = 2; else if (k.rep0 > 1u && off == k.rep0 - 1u) code = 3; }
-            if (code == 0) { offBase = off + 3u; k.rep2 = k.rep1; k.rep1 = k.rep0; k.rep0 = off; }
-            else {
-                offBase = code;
-                const uint32_t idx = code - 1u + (ll == 0u);
-                if (idx != 0) {
-                    const uint32_t cur = idx == 3 ? k.rep0 - 1u : (idx == 1 ? k.rep1 : k.rep2);
-                    if (idx != 1) k.rep2 = k.rep1;
-                    k.rep1 = k.rep0; k.rep0 = cur;
-                }
+        const uint32_t off = B2Z_CAND_OFF(sm.candTile[lane][w]);
+        if (l == B2Z_CAP) l = match_len(fw, segAbs + k.i - off, segAbs + k.i, sn - k.i, nWords);   // the full common prefix, to the segment end at most
+        const uint32_t ll = k.i - k.prevEnd;
+        uint32_t code = 0, offBase;
+        if (ll) { if (off == k.rep0) code = 1; else if (off == k.rep1) code = 2; else if (off == k.rep2) code = 3; }
+        else { if (off == k.rep1) code = 1; else if (off == k.rep2) code = 2; else if (k.rep0 > 1u && off == k.rep0 - 1u) code = 3; }
+        if (code == 0) { offBase = off + 3u; k.rep2 = k.rep1; k.rep1 = k.rep0; k.rep0 = off; }
+        else {
+            offBase = code;
+            const uint32_t idx = code - 1u + (ll == 0u);
+            if (idx != 0) {
+                const uint32_t cur = idx == 3 ? k.rep0 - 1u : (idx == 1 ? k.rep1 : k.rep2);
+                if (idx != 1) k.rep2 = k.rep1;
+                k.rep1 = k.rep0; k.rep0 = cur;
             }
-            outSeq[k.ns] = B2Z_PACK_SEQ(offBase, ll, l);
-            k.prevEnd = pos + l;
         }
-        k.ns++; k.i += l; k.lastEnd = s0 + k.i;
+        sm.recs[lane][k.np ^ (lane & 15u)] = B2Z_PACK_SEQ(offBase, ll, l);
+        k.np++; k.ns++; k.i += l; k.prevEnd = k.i;
     }
     return lits;
+}
+
+// the records the lanes hold in sm.recs, two lanes' runs per warp store (lane L's due at out + DP_LANE_SEQS L + its count before them);
+// the walk's writes must be synced
+__device__ __forceinline__ void dp_store_records(const DpWarpSmem& sm, DpWalk& k, uint32_t lane, uint64_t* __restrict__ out) {
+    static_assert(DP_PEND == 16u, "a half-warp stores one lane's run");
+    const uint32_t from = DP_LANE_SEQS * lane + k.ns - k.np, r = lane & 15u;
+#pragma unroll 4
+    for (uint32_t s = 0; s < 16u; s++) {
+        const uint32_t L = 2u * s + (lane >> 4);
+        const uint32_t cnt = __shfl_sync(B2Z_FULL, k.np, L), at = __shfl_sync(B2Z_FULL, from, L);
+        if (r < cnt) out[at + r] = sm.recs[L][r ^ (L & 15u)];
+    }
+    k.np = 0;
 }
 
 // the literals of one tile, lane by lane: lane L's are the bytes of its source row where bit `lits` is set, due at out + dst (its
@@ -202,7 +226,9 @@ __device__ __forceinline__ void dp_emit_literals(const DpWarpSmem& sm, uint32_t 
     }
 }
 
-__global__ void __launch_bounds__(B2Z_DP_WARPS * 32)
+// 4 CTAs (16 warps) per SM: with that budget ptxas keeps 124 registers, and the kernel runs faster than the 96-register, 20-warp
+// schedule it picks without the minimum
+__global__ void __launch_bounds__(B2Z_DP_WARPS * 32, 4)
 zstd_enc_dp_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g, const uint32_t* __restrict__ cand, uint8_t* __restrict__ choice,
                    uint64_t* __restrict__ seqs, uint32_t* __restrict__ nseq, uint8_t* __restrict__ lits, uint32_t* __restrict__ nlit,
                    uint32_t nBlockSlots) {
@@ -323,21 +349,24 @@ zstd_enc_dp_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
 
     const uint64_t* __restrict__ fw = reinterpret_cast<const uint64_t*>(fb);
     const uint32_t nWords = (n + 7u) >> 3;
-    const uint32_t* __restrict__ cnd = cndB + s0;
-    // ---- 3. count (tile 0's choices are still in shared memory from the last step of the programme: each lane's own row)
-    DpWalk k; k.i = 0; k.ns = 0; k.nl = 0; k.lastEnd = 0; k.rep0 = k.rep1 = k.rep2 = 0; k.prevEnd = 0;
+    // ---- 3. the walk (tile 0's choices and candidates are still in shared memory from the last step of the programme)
+    DpWalk k; k.i = 0; k.ns = 0; k.nl = 0; k.np = 0; k.prevEnd = 0; k.rep0 = k.rep1 = k.rep2 = 0;
     uint32_t qr[8];
     for (uint32_t t = 0; t < nTiles; t++) {
-        if (t) { dp_put_bytes(sm.chcTile, qr, lane); __syncwarp(); }
-        if (t + 1u < nTiles) dp_fetch_bytes(qr, chcB, bn, t + 1u, lane);
-        DP_TICK(DPC_CNT_LOAD);
-        dp_walk_tile<false>(sm, k, t, lane, sn, s0, fw, b0 + s0, nWords, cnd, nullptr);
+        if (t) { dp_put_bytes(sm.chcTile, qr, lane); dp_put_cand(sm, cr, lane); __syncwarp(); }
+        if (t + 1u < nTiles) { dp_fetch_bytes(qr, chcB, bn, t + 1u, lane); dp_fetch_cand(cr, cndB, bn, t + 1u, lane); }
+        DP_TICK(DPC_WALK_LOAD);
+        sm.srcTile[lane][t & 7u] = dp_walk_tile(sm, k, t, lane, sn, fw, b0 + s0, nWords);
         __syncwarp();
-        DP_TICK(DPC_CNT);
+        DP_TICK(DPC_WALK);
+        // the masks of tiles 8 u .. 8 u + 7 go where tile 8 u's choices were (each lane's 32 bytes: every tile's mask has a place there)
+        if ((t & 7u) == 7u || t + 1u == nTiles) dp_store_byte_tile(sm.srcTile, chcB, bn, t & ~7u, lane);
+        if (__any_sync(B2Z_FULL, k.np > DP_PEND / 2u) || t + 1u == nTiles) { dp_store_records(sm, k, lane, out); __syncwarp(); }
+        DP_TICK(DPC_WALK_STORE);
     }
     const uint32_t cntSeq = k.ns, cntLit = k.nl;
     // ---- 4. places: exclusive sums of the counts, exclusive maximum of the last match ends
-    uint32_t seqBase = cntSeq, litBase = cntLit, prevEnd = cntSeq ? k.lastEnd : 0u;
+    uint32_t seqBase = cntSeq, litBase = cntLit, prevEnd = cntSeq ? s0 + k.prevEnd : 0u;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
         const uint32_t a = __shfl_up_sync(B2Z_FULL, seqBase, d), c = __shfl_up_sync(B2Z_FULL, litBase, d), e = __shfl_up_sync(B2Z_FULL, prevEnd, d);
@@ -346,24 +375,55 @@ zstd_enc_dp_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom g,
     const uint32_t totSeq = __shfl_sync(B2Z_FULL, seqBase, 31), totLit = __shfl_sync(B2Z_FULL, litBase, 31);
     seqBase -= cntSeq; litBase -= cntLit;
     prevEnd = __shfl_up_sync(B2Z_FULL, prevEnd, 1); if (lane == 0) prevEnd = 0;
+    sm.runs[0][lane] = seqBase; sm.runs[1][lane] = DP_LANE_SEQS * lane - seqBase; sm.runs[2][lane] = s0 - prevEnd;
+    if (lane == 0) sm.runs[0][32] = totSeq;
+    __syncwarp();
     DP_TICK(DPC_SCAN);
-    // ---- 5. emit
-    k.i = 0; k.ns = 0; k.nl = 0; k.prevEnd = prevEnd;
-    dp_fetch_bytes(qr, chcB, bn, 0, lane);
+    // ---- 5. the move: record r of the block comes from its lane's staging run, r + runs[1][lane] (never below r, so a round's loads
+    // precede any store over them), and the lane's first record gets the literals before the segment start
+    {
+        constexpr uint32_t U = 8;
+        uint32_t L = 0;                                                        // the last lane whose run starts at or before r
+        for (uint32_t c = 0; c < totSeq; c += 32u * U) {
+            uint64_t v[U];
+            uint32_t patch[U];                                                 // added after the loads, which stay in flight together
+#pragma unroll
+            for (uint32_t u = 0; u < U; u++) {
+                const uint32_t r = c + 32u * u + lane;
+                patch[u] = 0;
+                if (r < totSeq) {
+                    while (sm.runs[0][L + 1u] <= r) L++;                       // runs[0][32] = totSeq ends the search
+                    v[u] = __ldcg(out + r + sm.runs[1][L]);
+                    if (r == sm.runs[0][L]) patch[u] = sm.runs[2][L];          // s0 - prevEnd more literals
+                }
+            }
+            __syncwarp();
+#pragma unroll
+            for (uint32_t u = 0; u < U; u++) {
+                const uint32_t r = c + 32u * u + lane;
+                if (r < totSeq) out[r] = v[u] + ((uint64_t)patch[u] << 28);   // litLength field
+            }
+        }
+    }
+    DP_TICK(DPC_MOVE);
+    // ---- 6. the literals: each tile's path literals from its mask, in place after the literals of the tiles before
+    uint32_t litAt = litBase;
     dp_fetch_bytes(sr, bs, bn, 0, lane);
-    dp_fetch_cand(cr, cndB, bn, 0, lane);
+    dp_fetch_bytes<true>(qr, chcB, bn, 0, lane);
     for (uint32_t t = 0; t < nTiles; t++) {
-        dp_put_bytes(sm.chcTile, qr, lane);
+        if ((t & 7u) == 0u) {
+            dp_put_bytes(sm.chcTile, qr, lane);
+            if (t + 8u < nTiles) dp_fetch_bytes<true>(qr, chcB, bn, t + 8u, lane);
+        }
         dp_put_bytes(sm.srcTile, sr, lane);
-        dp_put_cand(sm, cr, lane);
-        if (t + 1u < nTiles) { dp_fetch_bytes(qr, chcB, bn, t + 1u, lane); dp_fetch_bytes(sr, bs, bn, t + 1u, lane); dp_fetch_cand(cr, cndB, bn, t + 1u, lane); }
+        if (t + 1u < nTiles) dp_fetch_bytes(sr, bs, bn, t + 1u, lane);
         __syncwarp();
-        DP_TICK(DPC_EMIT_LOAD);
-        const uint32_t litAt = litBase + k.nl;
-        const uint32_t lits = dp_walk_tile<true>(sm, k, t, lane, sn, s0, fw, b0 + s0, nWords, cnd, out + seqBase);
+        DP_TICK(DPC_LIT_LOAD);
+        const uint32_t lits = sm.chcTile[lane][t & 7u];
         dp_emit_literals(sm, lits, litAt, lane, lit);
+        litAt += __popc(lits);
         __syncwarp();
-        DP_TICK(DPC_EMIT);
+        DP_TICK(DPC_LIT);
     }
     if (lane == 0) { nseq[bw] = totSeq; nlit[bw] = totLit; }
     DP_CLOCKS_FLUSH();

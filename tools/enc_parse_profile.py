@@ -7,13 +7,14 @@ Compresses --size-mib MiB of G2 text held on the device with compress_device (wh
 calls with the codec's stage counter stat(10) (stage G between two events), and one more call under torch.profiler for the
 per-kernel totals.  The card's name, power limit and SM clocks come from nvidia-smi in the same run.
 
-Rates: input GB/s = positions / stage G time; algorithmic DRAM GB/s counts per position the candidate word read twice (DP and
-emit passes, 8 B), the choice byte written once and read twice (3 B), the input byte read about 2.25 times (DP pass, emit pass,
-sampled histogram, literal copies) and about 1 B of sequences and literals written: 14.25 B.
+Rates: input GB/s = positions / stage G time; algorithmic DRAM GB/s counts per position the candidate word read twice (DP pass and
+walk, 8 B), the choice byte written once and read once and a 4-byte path-literal mask per 32 positions written and read back
+(2.25 B), the input byte read about 2.25 times (DP pass, literal pass, sampled histogram, match extensions) and about 2 B of
+sequences and literals (the sequence records are staged, read back and written again by the move): 14.5 B.
 
 --lib points the run at another build (B200Z_LIB).  A library built with -DB2Z_DP_CLOCKS also reports the phase split: every warp
-adds its clock64() cycles per phase (histogram, DP loads / DP / choice stores, count loads / count walk, scan, emit loads / emit
-walk) and the shares of their sum are printed.  The counters cost registers, so that build's own time is not stage G's time.
+adds its clock64() cycles per phase (histogram, DP loads / DP / choice stores, walk loads / walk / record and mask stores, scan,
+move of the records, literal-pass loads / literal stores) and the shares of their sum are printed.  The counters cost registers, so that build's own time is not stage G's time.
 Prints one JSON object (and writes it to --out).
 """
 import argparse
@@ -28,8 +29,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "7-zip-zstd_b200")
 sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 
-BYTES_PER_POSITION = 8 + 3 + 2.25 + 1.0
-PHASES = ["hist", "dp_load", "dp", "dp_store", "count_load", "count", "scan", "emit_load", "emit"]
+BYTES_PER_POSITION = 8 + 2.25 + 2.25 + 2.0
+PHASES = ["hist", "dp_load", "dp", "dp_store", "walk_load", "walk", "walk_store", "scan", "move", "lit_load", "lit"]
 
 
 def card():
