@@ -13,12 +13,12 @@
 // hops per CH positions; the result is the pure function of the frame's bytes that
 // oracle/zstd_enc_oracle.c:b2zo_zstd_candidates states position by position.
 //
-// Per iteration a position hashes its 16 bytes (loaded one iteration ahead), takes the turn, and then requests the next
-// iteration's bytes and both candidates' bytes together, one L2 round trip, before comparing either.  Level 3 (<4, 7, 0>, 896
-// threads): 56 registers, no spills; the GUARD = false loop is 159 SASS instructions per position (199 before, cuobjdump -sass).
-// Stage F per 4 GiB step of the bench: 43.3 -> 35.4 ms on an H100 80GB HBM3 (700 W, 1980 MHz).  The clock split of that build
-// (-DB2Z_F_CLOCKS) puts 70 % of a warp's cycles between the candidates' loads and their lengths, 15 % in the turn and under 2 %
-// waiting for it (DESIGN 2.2).
+// Per iteration a position takes the turn, compares the candidates it requested one iteration earlier, hashes the next
+// iteration's 16 bytes, and requests this iteration's two candidates together with the own bytes two iterations ahead (which an
+// L2 prefetch one iteration earlier has brought from DRAM), so a candidate's round trip runs while the group does its next turn.
+// Level 3 (<4, 7, 0>, 896 threads): 64 registers, no spills; the GUARD = false loop is 159 SASS instructions per position plus
+// the prefetch (cuobjdump -sass).  Stage F per 4 GiB step of the bench: 35.4 -> 31.0 ms on an H100 80GB HBM3 (700 W,
+// 1980 MHz); DESIGN 2.2.
 //
 // Output: one candidate word per position (B2Z_CAND: offset << 7 | length, 0 = none), consumed by stage G
 // (zstd_enc_dp.cu).  Replaces the finder half of zstd_double_fast.c:103-330 (ZSTD_compressBlock_doubleFast_noDict_generic:
@@ -44,24 +44,43 @@ __device__ __forceinline__ void turn_inputs_ready(uint32_t* slot, uint32_t iL, u
 #endif
 }
 
-// 16 bytes at any byte offset as four 32-bit words: five aligned 32-bit loads and four native funnel shifts (the 64-bit formulation
-// costs eight ALU instructions per 8 bytes).  GUARD: words at or beyond nW4 read as zero (only
-// the last frame of a buffer needs it: any other frame is followed by readable bytes, and a length is clipped to the frame anyway).
+// 16 bytes at any byte offset as four 32-bit words: the five aligned 32-bit words that hold them (W5, as loaded) and four native
+// funnel shifts (shr16; the 64-bit formulation costs eight ALU instructions per 8 bytes).  The two halves are apart so that a
+// load can be carried to a later iteration and shifted where it is used.  GUARD: words at or beyond nW4 read as zero (only the
+// last frame of a buffer needs it: any other frame is followed by readable bytes, and a length is clipped to the frame anyway).
 struct B16 { uint32_t x0, x1, x2, x3; };
+struct W5 { uint32_t t0, t1, t2, t3, t4; };
 static_assert(B2Z_CAP == 16, "stage F compares four 32-bit words");
-// (The funnel shift takes its amount mod 32, so o * 8 is the byte shift.)  ld16p: the words at w, shifted by sh, unguarded.
-__device__ __forceinline__ B16 ld16p(const uint32_t* __restrict__ w, uint32_t sh) {
-    const uint32_t t0 = __ldg(w), t1 = __ldg(w + 1), t2 = __ldg(w + 2), t3 = __ldg(w + 3), t4 = __ldg(w + 4);
-    B16 r; r.x0 = __funnelshift_r(t0, t1, sh); r.x1 = __funnelshift_r(t1, t2, sh); r.x2 = __funnelshift_r(t2, t3, sh); r.x3 = __funnelshift_r(t3, t4, sh);
-    return r;
+// The loads are coherent (ld.global.ca, L1-cached like __ldg): ptxas keeps those in front of a later bar.sync, where it would
+// sink non-coherent ones towards their use -- into the turn, or below it.
+__device__ __forceinline__ uint32_t ldca(const uint32_t* p) {
+#ifndef B2Z_CUEMU
+    return __ldca(p);
+#else
+    return __ldg(p);
+#endif
 }
 template <bool GUARD>
-__device__ __forceinline__ B16 ld16(const uint32_t* __restrict__ w4, uint32_t o, uint32_t nW4) {
-    const uint32_t a = o >> 2, sh = o * 8u;
-    if (!GUARD) return ld16p(w4 + a, sh);
-    const uint32_t t0 = a < nW4 ? __ldg(w4 + a) : 0u, t1 = a + 1u < nW4 ? __ldg(w4 + a + 1u) : 0u, t2 = a + 2u < nW4 ? __ldg(w4 + a + 2u) : 0u;
-    const uint32_t t3 = a + 3u < nW4 ? __ldg(w4 + a + 3u) : 0u, t4 = a + 4u < nW4 ? __ldg(w4 + a + 4u) : 0u;
-    B16 r; r.x0 = __funnelshift_r(t0, t1, sh); r.x1 = __funnelshift_r(t1, t2, sh); r.x2 = __funnelshift_r(t2, t3, sh); r.x3 = __funnelshift_r(t3, t4, sh);
+__device__ __forceinline__ W5 ld20(const uint32_t* __restrict__ w4, uint32_t a, uint32_t nW4) {
+    W5 r;
+    if (!GUARD) { r.t0 = ldca(w4 + a); r.t1 = ldca(w4 + a + 1u); r.t2 = ldca(w4 + a + 2u); r.t3 = ldca(w4 + a + 3u); r.t4 = ldca(w4 + a + 4u); return r; }
+    r.t0 = a < nW4 ? ldca(w4 + a) : 0u; r.t1 = a + 1u < nW4 ? ldca(w4 + a + 1u) : 0u; r.t2 = a + 2u < nW4 ? ldca(w4 + a + 2u) : 0u;
+    r.t3 = a + 3u < nW4 ? ldca(w4 + a + 3u) : 0u; r.t4 = a + 4u < nW4 ? ldca(w4 + a + 4u) : 0u;
+    return r;
+}
+// The own bytes are the first touch of the input, a DRAM round trip.  Their load shares its scoreboard with the candidates' loads
+// (ptxas puts every load of the loop on one), so the wait for the candidates after a turn would also wait for DRAM.  A prefetch
+// into L2 one iteration before the load (no register, no scoreboard) turns that load into an L2 hit like the candidates'.
+__device__ __forceinline__ void prefetch_l2(const uint32_t* p) {
+#ifndef B2Z_CUEMU
+    asm volatile("prefetch.global.L2 [%0];" :: "l"(p));
+#else
+    (void)p;
+#endif
+}
+// (the funnel shift takes its amount mod 32, so byte offset o gives sh = o * 8)
+__device__ __forceinline__ B16 shr16(const W5& t, uint32_t sh) {
+    B16 r; r.x0 = __funnelshift_r(t.t0, t.t1, sh); r.x1 = __funnelshift_r(t.t1, t.t2, sh); r.x2 = __funnelshift_r(t.t2, t.t3, sh); r.x3 = __funnelshift_r(t.t3, t.t4, sh);
     return r;
 }
 // common-prefix length (0..15) of two 16-byte strings, or a number above 16 when all 16 bytes agree (__ffs(0) - 1 wraps): the
@@ -83,7 +102,7 @@ struct FindCtx {
 // -DB2Z_F_CLOCKS (off by default; tools/enc_find_profile.py --build-clocks): every warp adds the clock64() cycles it spends in each
 // phase to f_clocks[]; b200z_find_clocks() reads and clears them.  Without the switch the ticks compile to nothing.
 //   wait: bar.sync of the turn (the previous group still holds it); turn: table reads, group barrier, atomics, hand-over;
-//   cand: from the candidates' loads to their compared lengths (mostly the L2 round trip); work: hash, prefetch, pack, store.
+//   cand: comparing the previous iteration's candidates (with whatever is left of their round trip); work: hash, the loads, store.
 enum { FC_WAIT, FC_TURN, FC_CAND, FC_WORK, FC_N };
 #ifdef B2Z_F_CLOCKS
 __device__ unsigned long long f_clocks[FC_N + 1];                             // [FC_N] = warps
@@ -92,12 +111,39 @@ __device__ unsigned long long f_clocks[FC_N + 1];                             //
 #define F_TICK(ph) do { } while (0)
 #endif
 
+// One position's candidates, carried from the turn that found them to the next one: where both candidates start, their offsets,
+// the lengths they may reach (0 for a candidate that failed its tag or window test), the position's own 16 bytes, and both
+// candidates' words as loaded.
+struct Pending { B16 own; W5 rL, rS; uint32_t cL, cS, offL, offS, mL, mS; };
+
+// both candidates' words of a pending position (a failed candidate starts at the position itself: no branch between the loads)
+template <bool FAST, bool GUARD>
+__device__ __forceinline__ void request(Pending& q, const uint32_t* __restrict__ w4, uint32_t nW4) {
+    if (!FAST) q.rL = ld20<GUARD>(w4, q.cL >> 2, nW4);
+    q.rS = ld20<GUARD>(w4, q.cS >> 2, nW4);
+}
+
+// the candidate word of a pending position (B2Z_CAND, 0 = none)
+template <bool FAST>
+__device__ __forceinline__ uint32_t cand_word(const Pending& q) {
+    const uint32_t lL = FAST ? 0u : prefix16(shr16(q.rL, q.cL * 8u), q.own), lS = prefix16(shr16(q.rS, q.cS * 8u), q.own);
+    const uint32_t lenL = FAST ? 0u : (lL < q.mL ? lL : q.mL), lenS = lS < q.mS ? lS : q.mS;
+    // the longer wins, the nearer of two equally long ones (offsets < 2^24: a frame is at most 2^B2Z_MAX_FRAMELOG bytes); a
+    // length below B2Z_DP_MINLEN makes the word 0 whichever side it came from
+    const uint32_t kL = (lenL << 24) | (~q.offL & 0xFFFFFFu), kS = (lenS << 24) | (~q.offS & 0xFFFFFFu);
+    const uint32_t k = kS > kL ? kS : kL, len = k >> 24;
+    return len >= B2Z_DP_MINLEN ? B2Z_CAND(len, ~k & 0xFFFFFFu) : 0u;
+}
+
 // the chunks of one frame (n bytes at w4, candidate words to out)
 //
-// Per position and iteration: hash the 16 bytes loaded one iteration ahead, take the turn, request the next iteration's bytes and
-// BOTH candidates' 16 bytes at once (no branch between the loads: a candidate that fails its tag or window test loads the position's
-// own bytes and gets length 0), then compare.  The output pointer and the own bytes' word index advance by a step per iteration;
-// the own bytes' shift is fixed per frame (p mod 4 never changes: a step is G * CH positions).
+// Per position and iteration: take the turn with the hash computed at the end of the previous iteration, compare the previous
+// iteration's candidates and store their word, hash the next iteration's 16 bytes (loaded one iteration earlier), then request
+// this iteration's candidates and the 16 bytes of the iteration after next.  A candidate's round trip so overlaps the group's
+// wait for its next turn instead of following the turn.  The hash comes before the loads because ptxas puts all of them on one
+// scoreboard: a wait for the own bytes also waits for every load issued before it.  The last iteration's candidates are
+// compared after the loop.  The output pointer and the own bytes' word index advance by a step per iteration; the own bytes'
+// shift is fixed per frame (p mod 4 never changes: a step is G * CH positions).
 template <int WPG, int G, int MODE, bool GUARD>
 __device__ __forceinline__ void find_frame(const FindCtx& c, const uint32_t* __restrict__ w4, uint32_t n, uint32_t* __restrict__ out
 #ifdef B2Z_F_CLOCKS
@@ -113,22 +159,27 @@ __device__ __forceinline__ void find_frame(const FindCtx& c, const uint32_t* __r
     // held in registers for the whole frame: without the opaque moves ptxas recomputes both in the loop (4 + 3 instructions)
     asm("mov.b64 %0, %0;" : "+l"(w4)); asm("mov.b32 %0, %0;" : "+r"(tagMask));
 #endif
-    // the index and the tag are the top HL + tagBits bits of the 64-bit product, and HL + tagBits <= 15 + (31 - 17) < 32
-    // (launch_zstd_enc_find checks it): only the high word of each product is formed.  (v << 24) * PRIME5 = v * (PRIME5 << 24).
     constexpr uint64_t PL = B2Z_PRIME8, PS = B2Z_PRIME5 << 24;
     const uint32_t shIL = 32u - HL, shIS = 32u - HS, shTL = 32u - HL - tagBits, shTS = 32u - HS - tagBits;
     const uint32_t nChunks = (n + CH - 1u) / CH, nIter = (nChunks + G - 1u) / G;
     uint32_t p = c.grp * CH + c.tg;
-    B16 vNext = ld16<true>(w4, p, nW4);
-    uint32_t aNext = (p >> 2) + STEPW / 4u;                               // the next iteration's own first word ...
-    const uint32_t shOwn = p * 8u;                                        // ... and byte shift (p mod 4 = tg mod 4 for the whole frame)
+    const uint32_t shOwn = p * 8u;                                        // the own bytes' shift (p mod 4 = tg mod 4 for the whole frame)
+    B16 own = shr16(ld20<true>(w4, p >> 2, nW4), shOwn);
+    W5 vNext = ld20<true>(w4, (p + STEPW) >> 2, nW4);                     // the next iteration's own bytes ...
+    uint32_t aNext = (p >> 2) + 2u * STEPW / 4u;                          // ... and the first word of the ones after them
+    uint32_t hl, hs;
+    // the index and the tag are the top HL + tagBits bits of the 64-bit product, and HL + tagBits <= 15 + (31 - 17) < 32
+    // (launch_zstd_enc_find checks it): only the high word of each product is formed.  (v << 24) * PRIME5 = v * (PRIME5 << 24).
+    auto hash = [&]() {
+        hl = (uint32_t)(((uint64_t)own.x0 * (uint32_t)PL) >> 32) + own.x0 * (uint32_t)(PL >> 32) + own.x1 * (uint32_t)PL;
+        hs = (uint32_t)(((uint64_t)own.x0 * (uint32_t)PS) >> 32) + own.x0 * (uint32_t)(PS >> 32) + own.x1 * (uint32_t)PS;
+    };
+    hash();
     uint32_t* __restrict__ o = out + p;
+    Pending q = {};                                                       // nothing pending before the first iteration (lengths 0)
     for (uint32_t it = 0; it < nIter; it++, p += STEPW, aNext += STEPW / 4u, o += STEPW) {
-        // ---- before the turn: the 16 bytes at p (loaded one iteration ahead), hashes, same-step groups
-        const B16 own = vNext;
+        // ---- before the turn: table indices and tags of the 16 bytes at p, same-step groups
         const bool hashable = p + 8u <= n;                                 // p >= n for the padding chunks of the last iteration
-        const uint32_t hl = (uint32_t)(((uint64_t)own.x0 * (uint32_t)PL) >> 32) + own.x0 * (uint32_t)(PL >> 32) + own.x1 * (uint32_t)PL;
-        const uint32_t hs = (uint32_t)(((uint64_t)own.x0 * (uint32_t)PS) >> 32) + own.x0 * (uint32_t)(PS >> 32) + own.x1 * (uint32_t)PS;
         const uint32_t iL = hl >> shIL, iS = hs >> shIS;
         const uint32_t tL = (hl >> shTL) & tagMask, tS = (hs >> shTS) & tagMask;
         const uint32_t mineL = ((p + 1u) << tagBits) | tL, mineS = ((p + 1u) << tagBits) | tS;
@@ -160,31 +211,30 @@ __device__ __forceinline__ void find_frame(const FindCtx& c, const uint32_t* __r
             if (lowL) eL = fromL;
             if (lowS) eS = fromS;
         }
-        // ---- after the turn: the next iteration's bytes and both candidates are requested before either is compared
-        if (GUARD) vNext = ld16<true>(w4, p + STEPW, nW4);
-        else vNext = ld16p(w4 + aNext, shOwn);
-        uint32_t word = 0;
-        if (hashable) {                                                    // (the branch also keeps ptxas from hoisting the loads into the turn)
-            const uint32_t offL = p - ((eL >> tagBits) - 1u), offS = p - ((eS >> tagBits) - 1u);
-            const bool okL = !FAST && hashable && eL && (eL & tagMask) == tL && offL <= W;
-            const bool okS = hashable && eS && (eS & tagMask) == tS && offS <= W && !(okL && offS == offL);   // not the long one's offset
-            const B16 cL = ld16<GUARD>(w4, p - (okL ? offL : 0u), nW4);
-            const B16 cS = ld16<GUARD>(w4, p - (okS ? offS : 0u), nW4);
-            // at most B2Z_CAP = 16 bytes are compared, never beyond the position's 4 KiB parse segment
-            const uint32_t segEnd = ((p | (B2Z_SEG - 1u)) + 1u) < n ? ((p | (B2Z_SEG - 1u)) + 1u) : n;
-            const uint32_t maxLen = (segEnd - p) < B2Z_CAP ? (segEnd - p) : B2Z_CAP;
-            const uint32_t lL = prefix16(cL, own), lS = prefix16(cS, own);
+        // ---- after the turn: the previous iteration's word (the branch keeps ptxas from moving the compare into the turn)
+        if (p - STEPW < n) {                                               // (p - STEPW wraps around in the first iteration)
+            const uint32_t word = cand_word<FAST>(q);
             F_TICK(FC_CAND);
-            const uint32_t mL = okL ? maxLen : 0u, mS = okS ? maxLen : 0u;
-            const uint32_t lenL = FAST ? 0u : (lL < mL ? lL : mL), lenS = lS < mS ? lS : mS;
-            // the longer wins, the nearer of two equally long ones (offsets < 2^24: a frame is at most 2^B2Z_MAX_FRAMELOG bytes); a
-            // length below B2Z_DP_MINLEN makes the word 0 whichever side it came from
-            const uint32_t kL = (lenL << 24) | (~offL & 0xFFFFFFu), kS = (lenS << 24) | (~offS & 0xFFFFFFu);
-            const uint32_t k = kS > kL ? kS : kL, len = k >> 24;
-            word = len >= B2Z_DP_MINLEN ? B2Z_CAND(len, ~k & 0xFFFFFFu) : 0u;
+            __stcs(o - STEPW, word);
         }
-        if (p < n) __stcs(o, word);                                        // streaming: the words are next read by another kernel
+        const uint32_t offL = p - ((eL >> tagBits) - 1u), offS = p - ((eS >> tagBits) - 1u);
+        const bool okL = !FAST && hashable && eL && (eL & tagMask) == tL && offL <= W;
+        const bool okS = hashable && eS && (eS & tagMask) == tS && offS <= W && !(okL && offS == offL);   // not the long one's offset
+        // at most B2Z_CAP = 16 bytes are compared, never beyond the position's 4 KiB parse segment
+        const uint32_t segEnd = ((p | (B2Z_SEG - 1u)) + 1u) < n ? ((p | (B2Z_SEG - 1u)) + 1u) : n;
+        const uint32_t maxLen = (segEnd - p) < B2Z_CAP ? (segEnd - p) : B2Z_CAP;
+        q.own = own; q.cL = p - (okL ? offL : 0u); q.cS = p - (okS ? offS : 0u); q.offL = offL; q.offS = offS;
+        q.mL = okL ? maxLen : 0u; q.mS = okS ? maxLen : 0u;                // (0 for a position that is not hashable)
+        // ---- the next iteration's hash, then the loads
+        own = shr16(vNext, shOwn);
+        hash();
+        vNext = GUARD ? ld20<true>(w4, (p + 2u * STEPW) >> 2, nW4) : ld20<false>(w4, aNext, 0u);
+        if (!GUARD) prefetch_l2(w4 + aNext + STEPW / 4u);                 // and the ones after those into L2 (see prefetch_l2)
+        request<FAST, GUARD>(q, w4, nW4);
     }
+    // the last iteration's candidates (p and o are one step past it)
+    const uint32_t word = cand_word<FAST>(q);
+    if (p - STEPW < n) __stcs(o - STEPW, word);
 }
 
 template <int WPG, int G, int MODE>
@@ -237,8 +287,9 @@ zstd_enc_find_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeom 
         for (uint32_t i = tid; i < c.tableWords / 4u; i += NT) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
         __syncthreads();
         F_TICK(FC_WORK);
-        // a frame followed by at least 4 KiB of the buffer needs no bounds checks on its loads (they reach at most 2 * 896 + 20 bytes
-        // past the frame: the prefetch of a padding chunk)
+        // a frame followed by at least 4 KiB of the buffer needs no bounds checks on its loads (they reach at most 3 * 896 + 20 bytes
+        // past the frame: the own bytes two iterations after a padding chunk; the L2 prefetch of the own bytes one iteration
+        // further reaches 4 * 896 bytes)
         if (srcSize - f0 - n >= 4096u) find_frame<WPG, G, MODE, false>(c, w4, n, out B2Z_F_CLOCK_ARGS);
         else find_frame<WPG, G, MODE, true>(c, w4, n, out B2Z_F_CLOCK_ARGS);
     }

@@ -12,7 +12,7 @@ the other, so a turn lasts stage F's time * SM clock / (turns per SM) -- with th
 
 --lib points the run at another build (B200Z_LIB).  A library built with -DB2Z_F_CLOCKS also reports the phase split: every warp
 adds its clock64() cycles per phase (wait: for its turn; turn: the table reads and atomics between the barriers; cand: the
-candidates' loads to their compared lengths; work: hash, prefetch, pack, store) and the shares of their sum are printed.  The
+compare of the previous iteration's candidates, with whatever is left of their round trip; work: hash, loads, pack, store) and the shares of their sum are printed.  The
 counters cost registers and instructions, so that build's own time is not stage F's time.
 Prints one JSON object (and writes it to --out).
 """
