@@ -22,7 +22,7 @@ struct DecFrame {
     uint64_t regen;         // D0: end offset of the frame in src; from D2 on: sum of block sizes
     uint32_t firstBlock, nBlocks;
     uint32_t checksum;      // 1 if a 4-byte content checksum follows the last block
-    uint32_t pad;           // D0: scratch (frame header bytes); from D2 on: index of the frame's first execution unit
+    uint32_t pad;           // D0: 1 = the end offset came from a size hint; from D2 on: index of the frame's first execution unit
     uint64_t endOff;        // offset just past the frame in src (the checksum, if any, is the 4 bytes before it)
     uint32_t jump;          // D2: 1 = the frame's matches are resolved by pointer jumping (stage J) instead of by execution units
     uint32_t nComp;         // D0: compressed blocks of the frame (the only ones that own literal / sequence scratch)
@@ -64,6 +64,95 @@ struct DecBlock {
 #define B2Z_DEC_JUMP_ROUNDS 32u      // pointer doubling: a chain of n links is resolved after ceil(log2 n) rounds, n < 2^31
 
 struct DecCounts { uint32_t nFrames, nBlocks, status, nUnits; uint64_t srcUsed; uint32_t maxFrameBlocks, nJump, nSlots, pad; };
+
+// ---------------------------------------------------------------- frame and block headers (RFC 8878 3.1.1)
+// One walk for the D0 prepass (zstd_dec.cu reads through its Src) and the host queries (zstd_dec_api.cu, through HostBytes).  A
+// reader has u8 / le24 / le32: little-endian values at a byte offset.
+#define B2Z_ZSTD_MAGIC 0xFD2FB528u
+#define B2Z_DERR_TRUNCATED 32u       // the walk only: the bytes end inside a frame.  D0 reports it as B2Z_DERR_CORRUPT; a host query
+                                     // over a stream read piece by piece waits for more bytes
+
+struct HostBytes {                   // bytes past the end read as 0, as past the end of the device's Src
+    const uint8_t* p; uint64_t size;
+    __host__ __device__ uint32_t u8(uint64_t off) const { return off < size ? p[off] : 0u; }
+    __host__ __device__ uint32_t le24(uint64_t off) const { return u8(off) | u8(off + 1) << 8 | u8(off + 2) << 16; }
+    __host__ __device__ uint32_t le32(uint64_t off) const { return le24(off) | u8(off + 3) << 24; }
+};
+
+// Whether the frame at ip, whose first 4 bytes are `magic`, is a skippable frame (magic 0x184D2A50 .. 0x184D2A5F); then *size = its
+// size with the 8-byte header, which may run past the end (8 when its size field is cut off)
+template <class R>
+__host__ __device__ inline bool zstd_skippable(const R& r, uint32_t magic, uint64_t ip, uint64_t srcSize, uint64_t* size) {
+    if ((magic & 0xFFFFFFF0u) != 0x184D2A50u) return false;
+    *size = srcSize - ip < 8 ? 8u : 8u + (uint64_t)r.le32(ip + 4);
+    return true;
+}
+
+// Block_Maximum_Size = min(Window_Size, 128 KiB) (RFC 8878 3.1.1.2.4)
+__host__ __device__ __forceinline__ uint64_t block_max(uint64_t windowSize) { return windowSize < 131072u ? windowSize : 131072u; }
+
+// status: 0, B2Z_DERR_TRUNCATED or B2Z_DERR_CORRUPT (reserved bit, window exponent above 31); the parse stops there.
+// unsupported: B2Z_DERR_UNSUPPORTED when a dictionary ID or a window above 1 GiB - 16 was met before that.  The decoder refuses such
+// frames, and the dictionary ID outranks a content size field cut short; the host queries describe them all the same.
+// blockMax: Block_Maximum_Size from the declared window (windowSize may be cut to the content size).
+struct ZstdFrameHdr { uint64_t contentSize, windowSize, blockMax; uint32_t checksum, hdrBytes, fcsBytes, status, unsupported; };
+
+// The frame header at ip, whose magic the caller has checked.  contentSize: ~0 when not declared (fcsBytes = 0).
+template <class R>
+__host__ __device__ inline ZstdFrameHdr zstd_frame_hdr(const R& r, uint64_t ip, uint64_t srcSize) {
+    ZstdFrameHdr h; h.contentSize = ~0ull; h.windowSize = 0; h.blockMax = 0; h.checksum = 0; h.hdrBytes = 0; h.fcsBytes = 0; h.status = 0; h.unsupported = 0;
+    if (srcSize - ip < 6) { h.status = B2Z_DERR_TRUNCATED; return h; }
+    const uint64_t ip0 = ip;
+    const uint32_t fhd = r.u8(ip + 4); ip += 5;
+    const uint32_t fcsFlag = fhd >> 6, single = (fhd >> 5) & 1u, didFlag = fhd & 3u;
+    h.checksum = (fhd >> 2) & 1u;
+    if (fhd & 8u) { h.status = B2Z_DERR_CORRUPT; return h; }
+    if (!single) {
+        const uint32_t wd = r.u8(ip++); const uint32_t wl = 10u + (wd >> 3);
+        if (wl > 31) { h.status = B2Z_DERR_CORRUPT; return h; }
+        h.windowSize = (1ull << wl) + ((1ull << wl) >> 3) * (wd & 7u);
+    }
+    const uint32_t didBytes = didFlag == 3 ? 4u : didFlag;
+    uint32_t did = 0; for (uint32_t i = 0; i < didBytes; i++) did |= r.u8(ip + i) << (8 * i);
+    ip += didBytes;
+    if (did) h.unsupported = B2Z_DERR_UNSUPPORTED;
+    h.fcsBytes = fcsFlag == 0 ? single : (fcsFlag == 1 ? 2u : (fcsFlag == 2 ? 4u : 8u));
+    if (srcSize < ip || srcSize - ip < h.fcsBytes) { h.status = B2Z_DERR_TRUNCATED; return h; }
+    if (h.fcsBytes) { uint64_t fcs = 0; for (uint32_t i = 0; i < h.fcsBytes; i++) fcs |= (uint64_t)r.u8(ip + i) << (8 * i); if (h.fcsBytes == 2) fcs += 256; h.contentSize = fcs; }
+    ip += h.fcsBytes;
+    if (single) h.windowSize = h.contentSize;
+    h.blockMax = block_max(h.windowSize);
+    if (!single && h.contentSize != ~0ull && h.contentSize < h.windowSize) h.windowSize = h.contentSize;     // no offset can exceed the content (zstd --long=31 on a small file)
+    if (h.windowSize > (1ull << 30) - 16) h.unsupported = B2Z_DERR_UNSUPPORTED;
+    h.hdrBytes = (uint32_t)(ip - ip0);
+    return h;
+}
+
+// The blocks of the frame at `off` whose header h parsed without fault, then its checksum.  emit(index, type, Block_Size field,
+// payload offset, payload bytes (RLE: 1)) for every block; a nonzero return stops the walk and becomes its status.  status: 0,
+// B2Z_DERR_TRUNCATED, B2Z_DERR_CORRUPT (reserved block type, a block over Block_Maximum_Size) or emit's; end: just past the frame.
+struct ZstdBlocks { uint64_t end; uint32_t nBlocks, status; };
+template <class R, class Emit>
+__host__ __device__ inline ZstdBlocks zstd_walk_blocks(const R& r, uint64_t off, uint64_t srcSize, const ZstdFrameHdr& h, Emit emit) {
+    ZstdBlocks w; w.end = 0; w.nBlocks = 0; w.status = 0;
+    uint64_t ip = off + h.hdrBytes;
+    for (;;) {
+        if (srcSize < ip || srcSize - ip < 3) { w.status = B2Z_DERR_TRUNCATED; return w; }
+        const uint32_t bh = r.le24(ip); ip += 3;
+        const uint32_t last = bh & 1u, type = (bh >> 1) & 3u, bsize = bh >> 3;
+        if (type == 3 || bsize > h.blockMax) { w.status = B2Z_DERR_CORRUPT; return w; }
+        const uint32_t cSize = type == 1 ? 1u : bsize;
+        if (srcSize - ip < cSize) { w.status = B2Z_DERR_TRUNCATED; return w; }
+        if ((w.status = emit(w.nBlocks, type, bsize, ip, cSize))) return w;
+        w.nBlocks++;
+        ip += cSize;
+        if (last) break;
+    }
+    if (h.checksum) { if (srcSize - ip < 4) { w.status = B2Z_DERR_TRUNCATED; return w; } ip += 4; }
+    w.end = ip;
+    return w;
+}
+struct ZstdEmitNone { __host__ __device__ uint32_t operator()(uint32_t, uint32_t, uint32_t, uint64_t, uint32_t) const { return 0; } };
 
 // stage D0: frame discovery (1 thread; hops over mcmilk size hints when present), then per-frame block indexing
 void launch_zstd_dec_find_frames(const uint8_t* src, uint64_t srcSize, DecFrame* frames, uint32_t frameCap, DecCounts* counts, bool useHints, cudaStream_t st);

@@ -103,83 +103,10 @@ __device__ SeqHdr parse_seq_hdr(const Src& S, uint64_t off, uint32_t avail) {
 //   D0b (thread/frame)  frame header + block count (and end-offset check)
 //   D0c (1 thread)      firstBlock = exclusive scan of the block counts
 //   D0d (thread/frame)  block table entries incl. where each block's entropy tables come from
-// Block_Maximum_Size = min(Window_Size, 128 KiB) (RFC 8878 3.1.1.2.4)
-__device__ __forceinline__ uint64_t block_max(uint64_t windowSize) { return windowSize < 131072u ? windowSize : 131072u; }
-struct FrameHdr { uint64_t contentSize, windowSize, blockMax; uint32_t checksum, hdrBytes, status; };     // blockMax: from the declared window
-__device__ FrameHdr parse_frame_hdr(const Src& S, uint64_t ip, uint64_t srcSize) {
-    FrameHdr h; h.status = 0; h.contentSize = ~0ull; h.windowSize = 0; h.blockMax = 0; h.checksum = 0; h.hdrBytes = 0;
-    if (srcSize - ip < 6) { h.status = B2Z_DERR_CORRUPT; return h; }
-    const uint64_t ip0 = ip;
-    const uint32_t fhd = S.u8(ip + 4); ip += 5;
-    const uint32_t fcsFlag = fhd >> 6, single = (fhd >> 5) & 1u, didFlag = fhd & 3u;
-    h.checksum = (fhd >> 2) & 1u;
-    if (fhd & 8u) { h.status = B2Z_DERR_CORRUPT; return h; }
-    if (!single) {
-        const uint32_t wd = S.u8(ip++); const uint32_t wl = 10u + (wd >> 3);
-        if (wl > 31) { h.status = B2Z_DERR_CORRUPT; return h; }
-        h.windowSize = (1ull << wl) + ((1ull << wl) >> 3) * (wd & 7u);
-    }
-    const uint32_t didBytes = didFlag == 3 ? 4u : didFlag;
-    uint32_t did = 0; for (uint32_t i = 0; i < didBytes; i++) did |= S.u8(ip + i) << (8 * i);
-    ip += didBytes;
-    if (did) { h.status = B2Z_DERR_UNSUPPORTED; return h; }
-    const uint32_t fcsBytes = fcsFlag == 0 ? single : (fcsFlag == 1 ? 2u : (fcsFlag == 2 ? 4u : 8u));
-    if (srcSize < ip || srcSize - ip < fcsBytes) { h.status = B2Z_DERR_CORRUPT; return h; }
-    if (fcsBytes) { uint64_t fcs = 0; for (uint32_t i = 0; i < fcsBytes; i++) fcs |= (uint64_t)S.u8(ip + i) << (8 * i); if (fcsBytes == 2) fcs += 256; h.contentSize = fcs; }
-    ip += fcsBytes;
-    if (single) h.windowSize = h.contentSize;
-    h.blockMax = block_max(h.windowSize);
-    if (!single && h.contentSize != ~0ull && h.contentSize < h.windowSize) h.windowSize = h.contentSize;     // no offset can exceed the content (zstd --long=31 on a small file)
-    if (h.windowSize > (1ull << 30) - 16) { h.status = B2Z_DERR_UNSUPPORTED; return h; }
-    h.hdrBytes = (uint32_t)(ip - ip0);
-    return h;
-}
-
-// Walk the block headers of one frame starting at `ip` (first block header). Returns the status; *nb = blocks,
-// *ipEnd = offset after the last block.  With `out` != null also fills the block entries.
-// blockMax: Block_Maximum_Size; no block's size field may exceed it.
-__device__ uint32_t walk_blocks(const Src& S, uint64_t ip, uint64_t srcSize, uint64_t blockMax, uint32_t* nbOut, uint64_t* ipEnd,
-                                DecBlock* out, uint32_t firstBlock, uint32_t frameIdx, uint32_t blockCap, uint32_t firstSlot = 0, uint32_t* nCompOut = nullptr) {
-    uint32_t nb = 0, nComp = 0; int32_t lastHuf = -1, lastTbl[3] = { -1, -1, -1 };
-    for (;;) {
-        if (srcSize < ip || srcSize - ip < 3) return B2Z_DERR_CORRUPT;
-        const uint32_t bh = S.le24(ip); ip += 3;
-        const uint32_t last = bh & 1u, type = (bh >> 1) & 3u, bsize = bh >> 3;
-        if (type == 3 || bsize > 131072u || bsize > blockMax) return B2Z_DERR_CORRUPT;
-        const uint32_t cSize = type == 1 ? 1u : bsize;
-        if (srcSize - ip < cSize) return B2Z_DERR_CORRUPT;
-        if (out) {
-            if (firstBlock + nb >= blockCap) return B2Z_DERR_TABLE_FULL;
-            const int32_t self = (int32_t)(firstBlock + nb);
-            DecBlock b; b.srcOff = ip; b.type = type; b.frame = frameIdx; b.hufSrc = -1; b.tblSrc[0] = b.tblSrc[1] = b.tblSrc[2] = -1;
-            b.regen = 0; b.nbSeq = 0; b.litSize = 0; b.status = 0; b.rawSize = 0; b.cSize = cSize; b.nearBehind = 0;
-            b.slot = type == 2 ? firstSlot + nComp : 0xFFFFFFFFu; b.pad4 = 0;              // only compressed blocks own literal / sequence scratch
-            if (type != 2) { b.rawSize = bsize; b.regen = bsize; }
-            else {
-                const LitHdr lh = parse_lit_hdr(S, ip, bsize);
-                if (!lh.ok) return B2Z_DERR_CORRUPT;
-                if (lh.type == 2) { b.hufSrc = self; lastHuf = self; }
-                else if (lh.type == 3) { if (lastHuf < 0) return B2Z_DERR_CORRUPT; b.hufSrc = lastHuf; }
-                const uint32_t so = lh.hdr + lh.csize;
-                const SeqHdr sh = parse_seq_hdr(S, ip + so, bsize - so);
-                if (!sh.ok) return B2Z_DERR_CORRUPT;
-                if (sh.nbSeq) {
-                    for (int t = 0; t < 3; t++) {
-                        const uint32_t mode = (sh.modes >> (6 - 2 * t)) & 3u;      // LL, OF, ML
-                        if (mode == 3) { if (lastTbl[t] < 0) return B2Z_DERR_CORRUPT; b.tblSrc[t] = lastTbl[t]; }
-                        else { b.tblSrc[t] = self; lastTbl[t] = self; }
-                    }
-                }
-            }
-            out[firstBlock + nb] = b;
-        }
-        nb++; nComp += type == 2;
-        ip += cSize;
-        if (last) break;
-    }
-    *nbOut = nb; *ipEnd = ip; if (nCompOut) *nCompOut = nComp;
-    return 0;
-}
+// The frame and block header walk is b2z_dec.h's.  D0 has the whole stream, so a frame cut short is corrupt; what makes a frame
+// unsupported was met before any fault of its header (the parse stops at the first), so it comes first.
+__device__ __forceinline__ uint32_t d0_status(uint32_t walk) { return walk == B2Z_DERR_TRUNCATED ? B2Z_DERR_CORRUPT : walk; }
+__device__ __forceinline__ uint32_t d0_frame_status(const ZstdFrameHdr& h) { return h.unsupported ? h.unsupported : d0_status(h.status); }
 
 // useHints: trust mcmilk's 12-byte size hints (a skippable frame 0x184D2A50 whose 4-byte payload is the compressed size of the zstd frame
 // behind it).  counts->nUnits (unused before stage D2) returns how many were trusted: when the stream then fails to index, the caller
@@ -192,12 +119,11 @@ __global__ void zstd_dec_find_frames_kernel(const uint8_t* __restrict__ src, uin
     while (ip < srcSize && !status) {
         if (srcSize - ip < 4) { status = B2Z_DERR_CORRUPT; break; }
         const uint32_t magic = S.le32(ip);
-        if ((magic & 0xFFFFFFF0u) == 0x184D2A50u) {
-            if (srcSize - ip < 8) { status = B2Z_DERR_CORRUPT; break; }
-            const uint64_t sz = S.le32(ip + 4);
-            if (srcSize - ip < 8 + sz) { status = B2Z_DERR_CORRUPT; break; }
+        uint64_t sz;
+        if (zstd_skippable(S, magic, ip, srcSize, &sz)) {
+            if (srcSize - ip < sz) { status = B2Z_DERR_CORRUPT; break; }
             // a size hint? (payload = compressed size of the zstd frame that follows; verified by D0b)
-            if (useHints && magic == 0x184D2A50u && sz == 4 && srcSize - ip >= 16 && S.le32(ip + 12) == 0xFD2FB528u) {
+            if (useHints && magic == 0x184D2A50u && sz == 12 && srcSize - ip >= 16 && S.le32(ip + 12) == B2Z_ZSTD_MAGIC) {
                 const uint64_t fsz = S.le32(ip + 8);
                 if (fsz >= 9 && srcSize - (ip + 12) >= fsz) {
                     if (nf >= frameCap) { status = B2Z_DERR_TABLE_FULL; break; }
@@ -207,19 +133,17 @@ __global__ void zstd_dec_find_frames_kernel(const uint8_t* __restrict__ src, uin
                     ip += 12 + fsz; continue;
                 }
             }
-            ip += 8 + sz; continue;
+            ip += sz; continue;
         }
-        if (magic != 0xFD2FB528u) { status = B2Z_DERR_CORRUPT; break; }
+        if (magic != B2Z_ZSTD_MAGIC) { status = B2Z_DERR_CORRUPT; break; }
         if (nf >= frameCap) { status = B2Z_DERR_TABLE_FULL; break; }
-        const FrameHdr h = parse_frame_hdr(S, ip, srcSize);
-        if (h.status) { status = h.status; break; }
-        uint32_t nb; uint64_t end;
-        status = walk_blocks(S, ip + h.hdrBytes, srcSize, h.blockMax, &nb, &end, nullptr, 0, nf, 0);
-        if (status) break;
-        if (h.checksum) { if (srcSize - end < 4) { status = B2Z_DERR_CORRUPT; break; } end += 4; }
-        DecFrame fr; fr.srcOff = ip; fr.dstOff = 0; fr.contentSize = ~0ull; fr.windowSize = 0; fr.regen = end; fr.firstBlock = 0; fr.nBlocks = nb; fr.checksum = 0; fr.pad = 0; fr.endOff = end; fr.jump = 0; fr.nComp = 0; fr.firstSlot = 0; fr.pad4 = 0;
+        const ZstdFrameHdr h = zstd_frame_hdr(S, ip, srcSize);
+        if ((status = d0_frame_status(h))) break;
+        const ZstdBlocks w = zstd_walk_blocks(S, ip, srcSize, h, ZstdEmitNone{});
+        if ((status = d0_status(w.status))) break;
+        DecFrame fr; fr.srcOff = ip; fr.dstOff = 0; fr.contentSize = ~0ull; fr.windowSize = 0; fr.regen = w.end; fr.firstBlock = 0; fr.nBlocks = w.nBlocks; fr.checksum = 0; fr.pad = 0; fr.endOff = w.end; fr.jump = 0; fr.nComp = 0; fr.firstSlot = 0; fr.pad4 = 0;
         frames[nf++] = fr;
-        ip = end;
+        ip = w.end;
     }
     counts->nFrames = nf; counts->nBlocks = 0; counts->status = status; counts->srcUsed = ip; counts->nUnits = hinted;
 }
@@ -229,12 +153,17 @@ __global__ void zstd_dec_count_blocks_kernel(const uint8_t* __restrict__ src, ui
     if (f >= nFrames) return;
     Src S; S.w = reinterpret_cast<const uint64_t*>(src); S.nWords = (srcSize + 7) >> 3; S.size = srcSize;
     DecFrame fr = frames[f];
-    const FrameHdr h = parse_frame_hdr(S, fr.srcOff, srcSize);
-    uint32_t status = h.status, nb = 0, nComp = 0; uint64_t end = 0;
-    if (!status) status = walk_blocks(S, fr.srcOff + h.hdrBytes, srcSize, h.blockMax, &nb, &end, nullptr, 0, f, 0, 0, &nComp);
-    if (!status && h.checksum) { if (srcSize - end < 4) status = B2Z_DERR_CORRUPT; else end += 4; }
-    if (!status && end != fr.regen) status = B2Z_DERR_CORRUPT;          // a size hint that does not match its frame
-    fr.contentSize = h.contentSize; fr.windowSize = h.windowSize; fr.checksum = h.checksum; fr.nBlocks = nb; fr.pad = h.hdrBytes; fr.nComp = nComp;
+    const ZstdFrameHdr h = zstd_frame_hdr(S, fr.srcOff, srcSize);
+    uint32_t status = d0_frame_status(h), nb = 0, nComp = 0;
+    if (!status) {
+        const ZstdBlocks w = zstd_walk_blocks(S, fr.srcOff, srcSize, h, [&](uint32_t, uint32_t type, uint32_t, uint64_t, uint32_t) { nComp += type == 2; return 0u; });
+        if ((status = d0_status(w.status))) nComp = 0;
+        else {
+            nb = w.nBlocks;
+            if (w.end != fr.regen) status = B2Z_DERR_CORRUPT;           // a size hint that does not match its frame
+        }
+    }
+    fr.contentSize = h.contentSize; fr.windowSize = h.windowSize; fr.checksum = h.checksum; fr.nBlocks = nb; fr.nComp = nComp;
     frames[f] = fr;
     if (status) atomicOr(&counts->status, status);
 }
@@ -250,17 +179,44 @@ __global__ void zstd_dec_scan_blocks_kernel(DecFrame* frames, uint32_t nFrames, 
     if (total > blockCap) counts->status |= B2Z_DERR_TABLE_FULL;
 }
 
+// The block table entries of one frame, and where each compressed block's entropy tables come from: treeless literals reuse the
+// frame's last Huffman table, repeat mode its last FSE table of the kind.
 __global__ void zstd_dec_fill_blocks_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, DecFrame* frames, uint32_t nFrames,
                                             DecBlock* blocks, uint32_t blockCap, DecCounts* counts) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nFrames || counts->status) return;
     Src S; S.w = reinterpret_cast<const uint64_t*>(src); S.nWords = (srcSize + 7) >> 3; S.size = srcSize;
     const DecFrame fr = frames[f];
-    uint32_t nb; uint64_t end;
-    const uint64_t blockMax = parse_frame_hdr(S, fr.srcOff, srcSize).blockMax;           // (fr.windowSize may be cut to the content size)
-    const uint32_t status = walk_blocks(S, fr.srcOff + fr.pad, srcSize, blockMax, &nb, &end, blocks, fr.firstBlock, f, blockCap, fr.firstSlot);
+    uint32_t nComp = 0; int32_t lastHuf = -1, lastTbl[3] = { -1, -1, -1 };
+    const ZstdFrameHdr h = zstd_frame_hdr(S, fr.srcOff, srcSize);
+    const ZstdBlocks w = zstd_walk_blocks(S, fr.srcOff, srcSize, h, [&](uint32_t k, uint32_t type, uint32_t bsize, uint64_t ip, uint32_t cSize) -> uint32_t {
+        if (fr.firstBlock + k >= blockCap) return B2Z_DERR_TABLE_FULL;
+        const int32_t self = (int32_t)(fr.firstBlock + k);
+        DecBlock b; b.srcOff = ip; b.type = type; b.frame = f; b.hufSrc = -1; b.tblSrc[0] = b.tblSrc[1] = b.tblSrc[2] = -1;
+        b.regen = 0; b.nbSeq = 0; b.litSize = 0; b.status = 0; b.rawSize = 0; b.cSize = cSize; b.nearBehind = 0;
+        b.slot = type == 2 ? fr.firstSlot + nComp++ : 0xFFFFFFFFu; b.pad4 = 0;              // only compressed blocks own literal / sequence scratch
+        if (type != 2) { b.rawSize = bsize; b.regen = bsize; }
+        else {
+            const LitHdr lh = parse_lit_hdr(S, ip, bsize);
+            if (!lh.ok) return B2Z_DERR_CORRUPT;
+            if (lh.type == 2) { b.hufSrc = self; lastHuf = self; }
+            else if (lh.type == 3) { if (lastHuf < 0) return B2Z_DERR_CORRUPT; b.hufSrc = lastHuf; }
+            const uint32_t so = lh.hdr + lh.csize;
+            const SeqHdr sh = parse_seq_hdr(S, ip + so, bsize - so);
+            if (!sh.ok) return B2Z_DERR_CORRUPT;
+            if (sh.nbSeq) {
+                for (int t = 0; t < 3; t++) {
+                    const uint32_t mode = (sh.modes >> (6 - 2 * t)) & 3u;      // LL, OF, ML
+                    if (mode == 3) { if (lastTbl[t] < 0) return B2Z_DERR_CORRUPT; b.tblSrc[t] = lastTbl[t]; }
+                    else { b.tblSrc[t] = self; lastTbl[t] = self; }
+                }
+            }
+        }
+        blocks[self] = b;
+        return 0u;
+    });
     frames[f].regen = 0; frames[f].pad = 0;
-    if (status) atomicOr(&counts->status, status);
+    if (w.status) atomicOr(&counts->status, d0_status(w.status));
 }
 
 // ---------------------------------------------------------------- bit readers (single lane)

@@ -8,8 +8,6 @@
 
 using namespace b2z;
 
-static inline uint32_t rd32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
-
 static int dec_status_to_rc(b200z_ctx* ctx, uint32_t st) {
     if (st & B2Z_DERR_TABLE_FULL) return fail(ctx, B200Z_E_UNSUPPORTED, "more frames/blocks than the decoder tables hold%s");
     if (st & B2Z_DERR_UNSUPPORTED) return fail(ctx, B200Z_E_UNSUPPORTED, "dictionary or window > 1 GiB frames are not supported%s");
@@ -19,48 +17,35 @@ static int dec_status_to_rc(b200z_ctx* ctx, uint32_t st) {
     return 0;
 }
 
+// Sums what the blocks of a frame regenerate: raw / RLE blocks their size field, a compressed block `compressed` bytes
+struct RegenSum {
+    uint64_t* sum; uint32_t compressed;
+    __host__ __device__ uint32_t operator()(uint32_t, uint32_t type, uint32_t bsize, uint64_t, uint32_t) const { *sum += type == 2 ? compressed : bsize; return 0; }
+};
+
 extern "C" {
 
 // Walk frame headers (and block headers) on the host: cheap, sequential, no entropy decoding.
 // Follows ZSTD_getFrameHeader / ZSTD_findFrameCompressedSize (C/zstd/zstd_decompress.c:482-600,702).
 int b200z_zstd_frame_info(const void* srcv, size_t srcSize, uint64_t* contentSize, uint32_t* nFrames) {
-    const uint8_t* ip = (const uint8_t*)srcv; const uint8_t* iend = ip + srcSize;
-    uint64_t total = 0; uint32_t frames = 0; int unknown = 0;
-    while (ip < iend) {
-        if (iend - ip < 4) return B200Z_E_CORRUPT;
-        const uint32_t magic = rd32(ip);
-        if ((magic & 0xFFFFFFF0u) == 0x184D2A50u) {
-            if (iend - ip < 8) return B200Z_E_CORRUPT;
-            const uint32_t sz = rd32(ip + 4);
-            if ((size_t)(iend - ip) < 8 + (size_t)sz) return B200Z_E_CORRUPT;
-            ip += 8 + sz; continue;
+    const HostBytes r{ (const uint8_t*)srcv, srcSize };
+    uint64_t ip = 0, total = 0; uint32_t frames = 0; bool unknown = false;
+    while (ip < srcSize) {
+        if (srcSize - ip < 4) return B200Z_E_CORRUPT;
+        const uint32_t magic = r.le32(ip);
+        uint64_t sz;
+        if (zstd_skippable(r, magic, ip, srcSize, &sz)) {
+            if (srcSize - ip < sz) return B200Z_E_CORRUPT;
+            ip += sz; continue;
         }
-        if (magic != 0xFD2FB528u) return B200Z_E_CORRUPT;
-        if (iend - ip < 6) return B200Z_E_CORRUPT;
-        const uint32_t fhd = ip[4]; ip += 5;
-        const uint32_t fcsFlag = fhd >> 6, single = (fhd >> 5) & 1, checksum = (fhd >> 2) & 1, didFlag = fhd & 3;
-        if (fhd & 8) return B200Z_E_CORRUPT;
-        if (!single) ip += 1;
-        static const int didBytes[4] = { 0, 1, 2, 4 };
-        ip += didBytes[didFlag];
-        const int fcsBytes = fcsFlag == 0 ? (int)single : (fcsFlag == 1 ? 2 : (fcsFlag == 2 ? 4 : 8));
-        if (iend - ip < fcsBytes) return B200Z_E_CORRUPT;
-        if (fcsBytes) { uint64_t fcs = 0; for (int i = 0; i < fcsBytes; i++) fcs |= (uint64_t)ip[i] << (8 * i); if (fcsBytes == 2) fcs += 256; total += fcs; }
-        else unknown = 1;
-        ip += fcsBytes;
-        for (;;) {
-            if (iend - ip < 3) return B200Z_E_CORRUPT;
-            const uint32_t bh = ip[0] | (ip[1] << 8) | (ip[2] << 16); ip += 3;
-            const uint32_t last = bh & 1, type = (bh >> 1) & 3, bsize = bh >> 3;
-            if (type == 3) return B200Z_E_CORRUPT;
-            const size_t adv = type == 1 ? 1 : bsize;
-            if ((size_t)(iend - ip) < adv) return B200Z_E_CORRUPT;
-            if (!fcsBytes && type != 2) total += bsize;          // lower bound only; flagged unknown below
-            ip += adv;
-            if (last) break;
-        }
-        if (checksum) { if (iend - ip < 4) return B200Z_E_CORRUPT; ip += 4; }
-        frames++;
+        if (magic != B2Z_ZSTD_MAGIC) return B200Z_E_CORRUPT;
+        const ZstdFrameHdr h = zstd_frame_hdr(r, ip, srcSize);
+        if (h.status) return B200Z_E_CORRUPT;
+        uint64_t lower = 0;                                          // raw and RLE blocks: a lower bound where no size is declared
+        const ZstdBlocks w = zstd_walk_blocks(r, ip, srcSize, h, RegenSum{ &lower, 0 });
+        if (w.status) return B200Z_E_CORRUPT;
+        if (h.fcsBytes) total += h.contentSize; else { total += lower; unknown = true; }
+        frames++; ip = w.end;
     }
     if (nFrames) *nFrames = frames;
     if (contentSize) *contentSize = total;
@@ -72,54 +57,34 @@ int b200z_zstd_frame_info(const void* srcv, size_t srcSize, uint64_t* contentSiz
 // piece).  *usedBytes = end of the last complete frame taken (skippable frames go with the frame that follows; trailing ones with
 // the frame before), *contentBound = bytes those frames decode to -- exact where a frame declares its size, else the sum over its
 // blocks of what a block can regenerate (raw / RLE: its size field, compressed: 128 KiB).  Stops before a frame that would take
-// the sum past maxContent unless it is the first one.  B200Z_E_CORRUPT: the bytes at a frame start are no frame.
+// the sum past maxContent unless it is the first one.  B200Z_E_CORRUPT: the bytes at a frame start are no frame, or a frame's headers
+// are malformed; the outputs still describe the complete frames in front of it.
 int b200z_zstd_frame_prefix(const void* srcv, size_t srcSize, uint64_t maxContent, size_t* usedBytes, uint64_t* contentBound, uint32_t* nFrames) {
-    const uint8_t* base = (const uint8_t*)srcv; const uint8_t* ip = base; const uint8_t* iend = ip + srcSize;
-    uint64_t total = 0; uint32_t frames = 0; size_t used = 0;
-    while (ip < iend) {
-        if (iend - ip < 4) break;
-        const uint32_t magic = rd32(ip);
-        if ((magic & 0xFFFFFFF0u) == 0x184D2A50u) {
-            if (iend - ip < 8) break;
-            const uint32_t sz = rd32(ip + 4);
-            if ((size_t)(iend - ip) < 8 + (size_t)sz) break;
-            ip += 8 + sz;
-            if (frames) used = (size_t)(ip - base);              // after a frame: belongs to what was taken; before the first: to the frame to come
+    const HostBytes r{ (const uint8_t*)srcv, srcSize };
+    uint64_t ip = 0, total = 0; uint32_t frames = 0; size_t used = 0; int rc = B200Z_OK;
+    while (ip < srcSize && srcSize - ip >= 4) {
+        const uint32_t magic = r.le32(ip);
+        uint64_t sz;
+        if (zstd_skippable(r, magic, ip, srcSize, &sz)) {
+            if (srcSize - ip < sz) break;
+            ip += sz;
+            if (frames) used = (size_t)ip;                          // after a frame: belongs to what was taken; before the first: to the frame to come
             continue;
         }
-        if (magic != 0xFD2FB528u) { if (usedBytes) *usedBytes = used; return B200Z_E_CORRUPT; }
-        if (iend - ip < 6) break;
-        const uint8_t* p = ip + 5; const uint32_t fhd = ip[4];
-        const uint32_t fcsFlag = fhd >> 6, single = (fhd >> 5) & 1, checksum = (fhd >> 2) & 1, didFlag = fhd & 3;
-        if (fhd & 8) { if (usedBytes) *usedBytes = used; return B200Z_E_CORRUPT; }
-        if (!single) p += 1;
-        p += didFlag == 3 ? 4 : didFlag;
-        const int fcsBytes = fcsFlag == 0 ? (int)single : (fcsFlag == 1 ? 2 : (fcsFlag == 2 ? 4 : 8));
-        if (iend - p < fcsBytes) break;
-        uint64_t fcs = 0; for (int i = 0; i < fcsBytes; i++) fcs |= (uint64_t)p[i] << (8 * i); if (fcsBytes == 2) fcs += 256;
-        p += fcsBytes;
-        uint64_t bound = 0; bool complete = false;
-        for (;;) {
-            if (iend - p < 3) break;
-            const uint32_t bh = p[0] | (p[1] << 8) | (p[2] << 16); p += 3;
-            const uint32_t last = bh & 1, type = (bh >> 1) & 3, bsize = bh >> 3;
-            if (type == 3) { if (usedBytes) *usedBytes = used; return B200Z_E_CORRUPT; }
-            const size_t adv = type == 1 ? 1 : bsize;
-            if ((size_t)(iend - p) < adv) break;
-            bound += type == 2 ? 131072u : bsize;
-            p += adv;
-            if (last) { complete = true; break; }
-        }
-        if (!complete) break;
-        if (checksum) { if (iend - p < 4) break; p += 4; }
-        const uint64_t content = fcsBytes ? fcs : bound;
+        if (magic != B2Z_ZSTD_MAGIC) { rc = B200Z_E_CORRUPT; break; }
+        const ZstdFrameHdr h = zstd_frame_hdr(r, ip, srcSize);
+        uint64_t bound = 0;
+        const ZstdBlocks w = h.status ? ZstdBlocks{ 0, 0, h.status }
+                                      : zstd_walk_blocks(r, ip, srcSize, h, RegenSum{ &bound, 131072u });
+        if (w.status) { if (w.status == B2Z_DERR_CORRUPT) rc = B200Z_E_CORRUPT; break; }
+        const uint64_t content = h.fcsBytes ? h.contentSize : bound;
         if (frames && total + content > maxContent) break;
-        total += content; frames++; ip = p; used = (size_t)(ip - base);
+        total += content; frames++; ip = w.end; used = (size_t)ip;
     }
     if (usedBytes) *usedBytes = used;
     if (contentBound) *contentBound = total;
     if (nFrames) *nFrames = frames;
-    return B200Z_OK;
+    return rc;
 }
 
 }  // extern "C"
@@ -221,38 +186,23 @@ int b200z_zstd_decompress_device(b200z_ctx* ctx, const void* d_src, size_t srcSi
 // Host-side split of a compressed stream into batches of whole frames (only when every frame declares its
 // content size): returns false if the stream cannot be split that way (the caller then decodes in one shot).
 static bool split_frames(const uint8_t* src, size_t srcSize, uint64_t targetOut, std::vector<HostBatch>& out) {
+    const HostBytes r{ src, srcSize };
     size_t ip = 0; HostBatch cur{0, 0, 0, true};
     while (ip < srcSize) {
         if (srcSize - ip < 4) return false;
-        const uint32_t magic = rd32(src + ip);
-        if ((magic & 0xFFFFFFF0u) == 0x184D2A50u) {
-            if (srcSize - ip < 8) return false;
-            const size_t sz = rd32(src + ip + 4);
-            if (srcSize - ip < 8 + sz) return false;
-            ip += 8 + sz; continue;                                  // hints/skippable data stay attached to the following frame
+        const uint32_t magic = r.le32(ip);
+        uint64_t sz;
+        if (zstd_skippable(r, magic, ip, srcSize, &sz)) {
+            if (srcSize - ip < sz) return false;
+            ip += sz; continue;                                      // hints/skippable data stay attached to the following frame
         }
-        if (magic != 0xFD2FB528u || srcSize - ip < 6) return false;
-        size_t p = ip + 5; const uint32_t fhd = src[ip + 4];
-        const uint32_t fcsFlag = fhd >> 6, single = (fhd >> 5) & 1, checksum = (fhd >> 2) & 1, didFlag = fhd & 3;
-        if (!single) p += 1;
-        p += didFlag == 3 ? 4 : didFlag;
-        const int fcsBytes = fcsFlag == 0 ? (int)single : (fcsFlag == 1 ? 2 : (fcsFlag == 2 ? 4 : 8));
-        if (!fcsBytes || srcSize < p + (size_t)fcsBytes) return false;
-        uint64_t fcs = 0; for (int i = 0; i < fcsBytes; i++) fcs |= (uint64_t)src[p + i] << (8 * i); if (fcsBytes == 2) fcs += 256;
-        p += fcsBytes;
-        for (;;) {
-            if (srcSize - p < 3) return false;
-            const uint32_t bh = src[p] | (src[p + 1] << 8) | (src[p + 2] << 16); p += 3;
-            const uint32_t last = bh & 1, type = (bh >> 1) & 3, bsize = bh >> 3;
-            if (type == 3) return false;
-            const size_t adv = type == 1 ? 1 : bsize;
-            if (srcSize - p < adv) return false;
-            p += adv;
-            if (last) break;
-        }
-        if (checksum) { if (srcSize - p < 4) return false; p += 4; }
-        ip = p;
-        cur.srcLen = ip - cur.srcOff; cur.outSize += fcs;
+        if (magic != B2Z_ZSTD_MAGIC) return false;
+        const ZstdFrameHdr h = zstd_frame_hdr(r, ip, srcSize);
+        if (h.status || !h.fcsBytes) return false;
+        const ZstdBlocks w = zstd_walk_blocks(r, ip, srcSize, h, ZstdEmitNone{});
+        if (w.status) return false;
+        ip = w.end;
+        cur.srcLen = ip - cur.srcOff; cur.outSize += h.contentSize;
         if (cur.outSize >= targetOut) { out.push_back(cur); cur = HostBatch{ ip, 0, 0, true }; }
     }
     if (cur.srcLen || cur.outSize) { cur.srcLen = srcSize - cur.srcOff; out.push_back(cur); }

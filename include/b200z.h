@@ -135,7 +135,9 @@ int b200z_zstd_frame_info(const void *src, size_t srcSize, uint64_t *contentSize
 /* For callers that read a packed stream piece by piece (the coder module's decoder): the complete frames at the start of a buffer
  * that may end inside a frame.  *usedBytes = end of the last complete frame taken, *contentBound = the bytes they decode to (exact
  * where declared, else an upper bound from the block headers: raw / RLE size fields, 128 KiB per compressed block); stops before a
- * frame that would take the sum past maxContent unless it is the first.  B200Z_E_CORRUPT if the bytes at a frame start are no frame. */
+ * frame that would take the sum past maxContent unless it is the first.  B200Z_E_CORRUPT if the bytes at a frame start are no frame
+ * or a frame's headers are malformed.  All three outputs are written on every return: on B200Z_E_CORRUPT they describe the complete
+ * frames in front of the damage. */
 int b200z_zstd_frame_prefix(const void *src, size_t srcSize, uint64_t maxContent, size_t *usedBytes, uint64_t *contentBound, uint32_t *nFrames);
 
 int b200z_zstd_decompress_device(b200z_ctx *ctx, const void *d_src, size_t srcSize,

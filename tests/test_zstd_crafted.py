@@ -330,6 +330,7 @@ def invalid_corpus():
     fr = C.Frame(window_log=10, fcs_bytes=0); fr.raw(b"y" * 1000); fr.compressed(b"abc", [(3, 4, 1100)]); bad.append(("compressed-block-decodes-over-window", fr.finish()[0], CORRUPT))
     fr = base(); fr.raw(b"tail"); bad.append(("missing-last-block", fr.finish(last=False)[0], CORRUPT))
     fr = C.Frame(window_log=16, fcs_bytes=4, fhd_extra=8); fr.raw(b"abc"); bad.append(("frame-header-reserved-bit", fr.finish()[0], CORRUPT))
+    fr = C.Frame(window_log=32, fcs_bytes=4); fr.raw(b"abc"); bad.append(("window-exponent-over-31", fr.finish()[0], CORRUPT))     # descriptor 0xB0
     fr = base(); fr.compressed(b"abc", [(3, 8, 5)], modes_extra=1, check=False); bad.append(("modes-reserved-bits", fr.finish()[0], CORRUPT))
     # content size and checksum
     fr = C.Frame(window_log=16, fcs_bytes=4); fr.raw(b"abc"); comp, _ = fr.finish(); b = bytearray(comp); b[6] += 1; bad.append(("content-size-mismatch", bytes(b), CORRUPT))
