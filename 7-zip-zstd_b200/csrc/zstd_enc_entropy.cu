@@ -8,9 +8,10 @@
 //      compares, one symbol per lane for normalisation and costs, the FSE spread numbered by ballots, the state fill
 //      ranked by __match_any_sync.  Blocks that need no FSE chain (RLE blocks, no sequences, over the bound) are finished
 //      here; every other block leaves an EntRec (header sizes, logs, the three encoding tables) in scratch.
-//   E2 (zstd_enc_chains_kernel, 30 chains per warp): lane 3b+t runs the FSE state chain of symbol type t (LL, OF, ML) of
-//      block b of the warp's 10; the three lanes of a block step together from the last sequence to the first and leave
-//      one 32-bit word per sequence: the three states' bits in stream order (OF, ML, LL; <= 26 bits) and their count.
+//      Its sequence pass also leaves the three codes of every sequence (LL | OF << 8 | ML << 16) in the block's word area.
+//   E2 (zstd_enc_chains_kernel, one block per lane, ENT_CHAIN_BLOCKS per one-warp CTA): a lane runs the LL, OF and ML state
+//      chains of its block together from the last sequence to the first, reading the code words, and writes over each one
+//      word per sequence: the three states' bits in stream order (OF, ML, LL; <= 26 bits) and their count.
 //   E3 (zstd_enc_seqbits_kernel, one warp per block): the sequence bitstream -- state word + LL/ML/OF extra bits per
 //      sequence, placed by prefix sum -- then the final states, the end mark, and the compressed-or-raw block choice.
 //
@@ -46,23 +47,33 @@ __device__ const int16_t d_OF_defNorm[29] = { 1,1,1,1,1,1,2,2,2,1,1,1,1,1,1,1,
 __device__ const uint8_t d_log2frac[32] = { 0, 11, 22, 33, 43, 53, 63, 72, 82, 91, 100, 108, 116, 125, 132, 140,
     148, 155, 162, 169, 176, 182, 189, 195, 201, 207, 213, 219, 225, 230, 236, 241 };
 
-__device__ __forceinline__ uint32_t ll_code(uint32_t ll) {
-    if (ll < 16) return ll;
-    if (ll < 24) return 16 + ((ll - 16) >> 1);
-    if (ll < 32) return 20 + ((ll - 24) >> 2);
-    if (ll < 48) return 22 + ((ll - 32) >> 3);
-    if (ll < 64) return 24;
-    return highbit32(ll) + 19;
-}
-__device__ __forceinline__ uint32_t ml_code(uint32_t m) {   // m = matchLength - 3
-    if (m < 32) return m;
-    if (m < 40) return 32 + ((m - 32) >> 1);
-    if (m < 48) return 36 + ((m - 40) >> 2);
-    if (m < 64) return 38 + ((m - 48) >> 3);
-    if (m < 96) return 40 + ((m - 64) >> 4);
-    if (m < 128) return 42;
-    return highbit32(m) + 36;
-}
+// length codes (RFC 8878 3.1.1.3.2.1.1): a table below 64 (literal lengths) and 128 (match lengths - 3), the highest set bit above
+__device__ const uint8_t d_LL_code[64] = { 0,1,2,3,4,5,6,7,8,9,10,11,12,13,14,15,16,16,17,17,18,18,19,19,20,20,20,20,21,21,21,21,
+    22,22,22,22,22,22,22,22,23,23,23,23,23,23,23,23,24,24,24,24,24,24,24,24,24,24,24,24,24,24,24,24 };
+__device__ const uint8_t d_ML_code[128] = { 0,1,2,3,4,5,6,7,8,9,10,11,12,13,14,15,16,17,18,19,20,21,22,23,24,25,26,27,28,29,30,31,
+    32,32,33,33,34,34,35,35,36,36,36,36,37,37,37,37,38,38,38,38,38,38,38,38,39,39,39,39,39,39,39,39,
+    40,40,40,40,40,40,40,40,40,40,40,40,40,40,40,40,41,41,41,41,41,41,41,41,41,41,41,41,41,41,41,41,
+    42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42,42 };
+__device__ __forceinline__ uint32_t ll_code(uint32_t ll) { return ll < 64 ? (uint32_t)d_LL_code[ll] : highbit32(ll) + 19u; }
+__device__ __forceinline__ uint32_t ml_code(uint32_t m) { return m < 128 ? (uint32_t)d_ML_code[m] : highbit32(m) + 36u; }   // m = matchLength - 3
+
+// -DB2Z_E_CLOCKS (off by default; tools/enc_entropy_profile.py --build-clocks): lane 0 of every E1 and E2 warp adds the clock64()
+// cycles its warp spends in each phase to e_clocks[]; b200z_e_clocks() reads and clears them.  E1: literal histogram (with the
+// RLE-block test), Huffman build and description, literal streams (or the raw / RLE literals), sequence pass (code histograms),
+// the three table choices, table hand-off (or the block's finish).  E2: table staging, code loads, chain steps, word stores.
+// Without the switch the ticks compile to nothing.
+enum { E1C_LITHIST, E1C_HUF, E1C_LITSTREAMS, E1C_SEQPASS, E1C_TABLES, E1C_HANDOFF, E1C_N };
+enum { E2C_STAGE, E2C_LOAD, E2C_STEP, E2C_STORE, E2C_N };
+#if defined(B2Z_E_CLOCKS) && !defined(B2Z_CUEMU)
+__device__ unsigned long long e_clocks[E1C_N + E2C_N];                  // E1's phases, then E2's
+#define E_CLOCKS_START(n) unsigned long long ec_[n] = {}; long long ecLast_ = clock64()
+#define E_TICK(ph) do { const long long now_ = clock64(); ec_[ph] += (unsigned long long)(now_ - ecLast_); ecLast_ = now_; } while (0)
+#define E_CLOCKS_FLUSH(base, n) do { if (lane == 0) for (int p_ = 0; p_ < (n); p_++) atomicAdd(&e_clocks[(base) + p_], ec_[p_]); } while (0)
+#else
+#define E_CLOCKS_START(n) do { } while (0)
+#define E_TICK(ph) do { } while (0)
+#define E_CLOCKS_FLUSH(base, n) do { } while (0)
+#endif
 
 __device__ __forceinline__ uint32_t warp_sum(uint32_t v) {
     for (int d = 16; d; d >>= 1) v += __shfl_xor_sync(B2Z_FULL, v, d);
@@ -125,7 +136,7 @@ struct EntRec {
     EntTables tab;
 };
 static_assert(sizeof(EntTables) % 16 == 0 && sizeof(EntRec) % 16 == 0 && offsetof(EntRec, tab) % 16 == 0, "EntRec is copied in 16-byte units");
-#define ENT_SCRATCH_STRIDE ((size_t)sizeof(EntRec) + (size_t)B2Z_MAXSEQ * 4u)   // record, then one state word per sequence
+#define ENT_SCRATCH_STRIDE ((size_t)sizeof(EntRec) + (size_t)B2Z_MAXSEQ * 4u)   // record, then one word per sequence (E1: codes, E2: states)
 static_assert(sizeof(EntRec) + (size_t)B2Z_MAXSEQ * 4u <= (size_t)B2Z_BLOCK * 4u, "stage E scratch must fit the block's candidate words");
 
 // ---------------------------------------------------------------- lane-0 bit writer to global memory
@@ -451,14 +462,22 @@ struct Stager {
 // Huffman-encode literals [a, b) as one backward stream at st.out, 4 literals per lane and 128 per step; returns stream bytes
 __device__ uint32_t huf_encode_stream(WarpWS* ws, Stager& st, const uint8_t* __restrict__ lit, uint32_t a, uint32_t b, uint32_t lane) {
     uint8_t* start = st.out;
+    uint32_t cur[4];                                             // lane's literals hi-1-4*lane .. hi-4-4*lane, loaded a step ahead
+#pragma unroll
+    for (uint32_t j = 0; j < 4; j++) { const uint32_t k = lane * 4u + j; cur[j] = k < b - a ? lit[b - 1u - k] : 0u; }
     for (uint32_t hi = b; hi > a;) {
-        const uint32_t cnt = (hi - a) < 128u ? (hi - a) : 128u;
-        uint64_t code = 0; uint32_t nb = 0;                      // lane's literals hi-1-4*lane .. hi-4-4*lane, <= 44 bits
+        const uint32_t cnt = (hi - a) < 128u ? (hi - a) : 128u, hn = hi - cnt;
+        uint32_t nxt[4];
+#pragma unroll
+        for (uint32_t j = 0; j < 4; j++) { const uint32_t k = lane * 4u + j; nxt[j] = k < hn - a ? lit[hn - 1u - k] : 0u; }
+        uint64_t code = 0; uint32_t nb = 0;                      // <= 44 bits
 #pragma unroll
         for (uint32_t j = 0; j < 4; j++) {
             const uint32_t k = lane * 4u + j;
-            if (k < cnt) { const uint32_t s = lit[hi - 1u - k]; code |= (uint64_t)ws->hufCode[s] << nb; nb += ws->hufLen[s]; }
+            if (k < cnt) { const uint32_t s = cur[j]; code |= (uint64_t)ws->hufCode[s] << nb; nb += ws->hufLen[s]; }
         }
+#pragma unroll
+        for (uint32_t j = 0; j < 4; j++) cur[j] = nxt[j];
         uint32_t total; const uint32_t off = warp_excl_scan(nb, lane, &total);
         st.put(st.bits + off, code, 0, nb);
         st.bits += total; hi -= cnt;
@@ -556,6 +575,7 @@ zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
     __shared__ WarpWS wsAll[B2Z_ENT_WARPS];
     const uint32_t lane = threadIdx.x & 31u, wib = threadIdx.x >> 5;
     WarpWS* ws = &wsAll[wib];
+    E_CLOCKS_START(E1C_N);
     for (uint32_t blk = blockIdx.x * B2Z_ENT_WARPS + wib; blk < nBlocks; blk += gridDim.x * B2Z_ENT_WARPS) {
         const BlockGeom bg = block_geom(g, srcSize, blk);
         const uint32_t blkSize = bg.blkSize, last = bg.last;
@@ -581,18 +601,29 @@ zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
         // =========================== literals section
         for (uint32_t i = lane; i < 256; i += 32) ws->hist[i] = 0;
         __syncwarp();
-        for (uint32_t i = lane * 4; i < nlit; i += 128) {
-            const uint32_t v = *reinterpret_cast<const uint32_t*>(lit + i);   // block literal area is 4-byte aligned, in-bounds (<= blkSize rounded)
-            const uint32_t k = nlit - i;
-            atomicAdd(&ws->hist[v & 255u], 1u);
-            if (k > 1) atomicAdd(&ws->hist[(v >> 8) & 255u], 1u);
-            if (k > 2) atomicAdd(&ws->hist[(v >> 16) & 255u], 1u);
-            if (k > 3) atomicAdd(&ws->hist[v >> 24], 1u);
+        {   // 16 bytes per lane and 512 per step, the next step's vector in flight: a block's literal area starts at a multiple of
+            // 2^17 and has room for the vector that holds its last literal
+            const uint4* lit4 = reinterpret_cast<const uint4*>(lit);
+            const uint32_t nv = (nlit + 15u) >> 4;
+            uint4 cur = lane < nv ? lit4[lane] : make_uint4(0, 0, 0, 0);
+            for (uint32_t v0 = 0; v0 < nv; v0 += 32) {
+                const uint32_t vi = v0 + lane;
+                const uint4 nxt = vi + 32u < nv ? lit4[vi + 32u] : make_uint4(0, 0, 0, 0);
+                if (vi < nv) {
+                    const uint32_t w[4] = { cur.x, cur.y, cur.z, cur.w };
+                    const uint32_t k = nlit - 16u * vi;              // literals left from this vector's first byte
+#pragma unroll
+                    for (uint32_t j = 0; j < 16; j++)
+                        if (j < k) atomicAdd(&ws->hist[(w[j >> 2] >> (8u * (j & 3u))) & 255u], 1u);
+                }
+                cur = nxt;
+            }
         }
         __syncwarp();
         uint32_t ns = 0;
         for (uint32_t i = lane; i < 256; i += 32) ns += ws->hist[i] != 0;
         ns = warp_sum(ns);
+        E_TICK(E1C_LITHIST);
 
         const uint32_t rawHdr = nlit < 32 ? 1u : (nlit < 4096 ? 2u : 3u);
         uint32_t litSecSize = 0;
@@ -616,6 +647,7 @@ zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
             uint32_t T = 0;
             for (uint32_t i = lane; i < 256; i += 32) T += ws->hist[i] * ws->hufLen[i];
             T = warp_sum(T);
+            E_TICK(E1C_HUF);
             const uint32_t est = ts + (four ? 6u : 0u) + ((T + 7u) >> 3) + (four ? 4u : 1u);
             if (ts && lh + est < rawHdr + nlit) {
                 uint8_t* p = body + lh + ts;
@@ -653,6 +685,7 @@ zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
             litSecSize = rawHdr + nlit;
         }
         __syncwarp();
+        E_TICK(E1C_LITSTREAMS);
 
         // =========================== sequences section: header and tables
         uint8_t* sp = body + litSecSize;
@@ -669,22 +702,37 @@ zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
             uint32_t* cLL = ws->hist; uint32_t* cOF = ws->hist + 64; uint32_t* cML = ws->hist + 128;
             for (uint32_t i = lane; i < 192; i += 32) ws->hist[i] = 0;
             __syncwarp();
+            // the three codes of every sequence, LL | OF << 8 | ML << 16, into the block's word area for E2
+            uint32_t* codeOut = reinterpret_cast<uint32_t*>(scratch + (size_t)blk * ENT_SCRATCH_STRIDE + sizeof(EntRec));
             uint32_t extra = 0;                                   // sum of raw extra bits (for the size bound)
-            for (uint32_t i0 = 0; i0 < nbSeq; i0 += 128) {        // four records per lane in flight
-                uint64_t v[4];
+            uint64_t v[4];                                        // four records per lane, the next four in flight
 #pragma unroll
-                for (uint32_t m = 0; m < 4; m++) { const uint32_t i = i0 + 32u * m + lane; v[m] = i < nbSeq ? sq[i] : 0ull; }
+            for (uint32_t m = 0; m < 4; m++) { const uint32_t i = 32u * m + lane; v[m] = i < nbSeq ? sq[i] : 0ull; }
+            for (uint32_t i0 = 0; i0 < nbSeq; i0 += 128) {
+                uint64_t nx[4];
+#pragma unroll
+                for (uint32_t m = 0; m < 4; m++) { const uint32_t i = i0 + 128u + 32u * m + lane; nx[m] = i < nbSeq ? sq[i] : 0ull; }
 #pragma unroll
                 for (uint32_t m = 0; m < 4; m++) {
                     const uint64_t s = v[m];
-                    if (!s) continue;                             // past the end (a record is never 0)
-                    const uint32_t cl = ll_code(B2Z_SEQ_LL(s)), cm = ml_code(B2Z_SEQ_ML(s) - 3u), co = highbit32(B2Z_SEQ_OFFBASE(s));
-                    atomicAdd(&cLL[cl], 1u); atomicAdd(&cML[cm], 1u); atomicAdd(&cOF[co], 1u);
-                    extra += d_LL_bits[cl] + d_ML_bits[cm] + co;
+                    const bool ok = s != 0;                       // past the end: a record is never 0
+                    const uint32_t cl = ok ? ll_code(B2Z_SEQ_LL(s)) : 255u, cm = ok ? ml_code(B2Z_SEQ_ML(s) - 3u) : 255u, co = ok ? highbit32(B2Z_SEQ_OFFBASE(s)) : 255u;
+                    // one add per distinct code of the 32 (a few codes take most sequences)
+                    const uint32_t gl = __match_any_sync(B2Z_FULL, cl), gm = __match_any_sync(B2Z_FULL, cm), go = __match_any_sync(B2Z_FULL, co);
+                    if (ok) {
+                        codeOut[i0 + 32u * m + lane] = cl | (co << 8) | (cm << 16);
+                        if (lane == (uint32_t)__ffs((int)gl) - 1u) atomicAdd(&cLL[cl], (uint32_t)__popc(gl));
+                        if (lane == (uint32_t)__ffs((int)gm) - 1u) atomicAdd(&cML[cm], (uint32_t)__popc(gm));
+                        if (lane == (uint32_t)__ffs((int)go) - 1u) atomicAdd(&cOF[co], (uint32_t)__popc(go));
+                        extra += d_LL_bits[cl] + d_ML_bits[cm] + co;
+                    }
                 }
+#pragma unroll
+                for (uint32_t m = 0; m < 4; m++) v[m] = nx[m];
             }
             extra = warp_sum(extra);
             __syncwarp();
+            E_TICK(E1C_SEQPASS);
             FseCT* ctL = &ws->u.fse.ct[0]; FseCT* ctO = &ws->u.fse.ct[1]; FseCT* ctM = &ws->u.fse.ct[2];
             uint8_t* tp = sp + seqSecSize + 1;
             uint32_t mL, mO, mM;
@@ -693,6 +741,7 @@ zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
             tp += choose_seq_table(ws, ctM, tp, cML, nbSeq, 52, 9, d_ML_defNorm, 52, 6, &mM, lane);
             if (lane == 0) sp[seqSecSize] = (uint8_t)((mL << 6) | (mO << 4) | (mM << 2));
             seqSecSize += 1 + (uint32_t)(tp - (sp + seqSecSize + 1));
+            E_TICK(E1C_TABLES);
             const uint64_t upper = (uint64_t)nbSeq * (ctL->log + ctO->log + ctM->log) + 1ull + extra;
             overCap = (uint64_t)litSecSize + seqSecSize + ((upper + 7ull) >> 3) > B2Z_BODY_CAP;
             if (!overCap) {                                       // hand the tables to E2 and the sizes to E3
@@ -705,6 +754,7 @@ zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
                 }
                 if (lane == 0) { rec->run = 1; rec->bodyHead = litSecSize + seqSecSize; rec->logs = ctL->log | (ctO->log << 8) | (ctM->log << 16); }
                 __syncwarp();
+                E_TICK(E1C_HANDOFF);
                 continue;
             }
         }
@@ -712,84 +762,112 @@ zstd_enc_tables_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
         const uint32_t outSize = finish_block(out, bsrc, blkSize, last, litSecSize + seqSecSize, overCap, lane);
         if (lane == 0) { slotSize[blk] = outSize; rec->run = 0; }
         __syncwarp();
+        E_TICK(E1C_HANDOFF);
     }
+    E_CLOCKS_FLUSH(0, E1C_N);
 }
 
-// ---------------------------------------------------------------- E2: the FSE state chains, 30 per warp
-// The sequence records are read a chunk at a time by the whole warp (ENT_CHAIN_SEQS per block, all loads in flight together)
-// and reduced to their three codes in shared memory, so the chains themselves wait on shared memory only.
-#define ENT_CHAIN_BLOCKS 10
-#define ENT_CHAIN_SEQS   48
-#define ENT_CHAIN_LOADS  (ENT_CHAIN_BLOCKS * ENT_CHAIN_SEQS / 32)
+// ---------------------------------------------------------------- E2: the FSE state chains, one block per lane
+// Lane j of a warp codes block blk0 + j alone: its LL, OF and ML states from the last sequence to the first, three independent
+// recurrences in one thread (the serial encoder's order), with the group's tables in the warp's dynamic shared memory.  It reads
+// the code words E1 left in the block's word area (LL | OF << 8 | ML << 16), four per 16-byte vector and ENT_CHAIN_VECS vectors
+// per round with the next round's in flight, and writes each sequence's state word over its code word: the three states' bits in
+// stream order (OF, ML, LL; <= 26 bits) and their count on top.  The last sequence only sets the initial states: its word is 0.
+// Lanes without a block to code (E1 finished it, or the group ends) and lanes whose block has run out of sequences idle.
+#define ENT_CHAIN_BLOCKS 16                                      // blocks per one-warp CTA, one per lane (lanes 16-31 idle: 4 CTAs
+                                                                 // per SM beat 32 blocks and 2 CTAs per SM, DESIGN §2.3)
+#define ENT_CHAIN_VECS   4                                       // code vectors per lane per round
+#define ENT_CHAIN_SMEM   ((size_t)ENT_CHAIN_BLOCKS * sizeof(EntTables))
+__device__ __forceinline__ uint32_t fse_first_state(const uint16_t* stT, uint2 e) {
+    const uint32_t nb = (e.x + (1u << 15)) >> 16;
+    return stT[(((nb << 16) - e.x) >> nb) + e.y];
+}
+__device__ __forceinline__ uint32_t fse_step(const uint16_t* stT, uint2 e, uint32_t& state, uint32_t& nbits) {
+    nbits = (state + e.x) >> 16;
+    const uint32_t bits = state & ((1u << nbits) - 1u);
+    state = stT[(state >> nbits) + e.y];
+    return bits;
+}
 __global__ void __launch_bounds__(32)
-zstd_enc_chains_kernel(const uint64_t* __restrict__ seqs, const uint32_t* __restrict__ nseqArr, uint8_t* __restrict__ scratch, uint32_t nBlocks) {
-    __shared__ EntTables tabs[ENT_CHAIN_BLOCKS];
-    __shared__ uint32_t codes[ENT_CHAIN_BLOCKS][ENT_CHAIN_SEQS];   // LL | OF << 8 | ML << 16 of walk steps k0 .. k0 + 47
-    __shared__ uint32_t nsq[ENT_CHAIN_BLOCKS];
-    const uint32_t lane = threadIdx.x, b = lane / 3u, t = lane - 3u * b;
+zstd_enc_chains_kernel(const uint32_t* __restrict__ nseqArr, uint8_t* __restrict__ scratch, uint32_t nBlocks) {
+    B2Z_DYN_SMEM(EntTables, tabs);
+    const uint32_t lane = threadIdx.x;
+    E_CLOCKS_START(E2C_N);
     for (uint32_t blk0 = blockIdx.x * ENT_CHAIN_BLOCKS; blk0 < nBlocks; blk0 += gridDim.x * ENT_CHAIN_BLOCKS) {
-        const uint32_t nb = nBlocks - blk0 < ENT_CHAIN_BLOCKS ? nBlocks - blk0 : ENT_CHAIN_BLOCKS;
-        // stage the group's tables (whole EntTables, 16 bytes per lane per step)
-        for (uint32_t j = 0; j < nb; j++) {
-            const EntRec* r = reinterpret_cast<const EntRec*>(scratch + (size_t)(blk0 + j) * ENT_SCRATCH_STRIDE);
-            if (!r->run) continue;
-            const uint4* s4 = reinterpret_cast<const uint4*>(&r->tab);
+        const uint32_t blk = blk0 + lane;
+        EntRec* rec = reinterpret_cast<EntRec*>(scratch + (size_t)blk * ENT_SCRATCH_STRIDE);
+        const bool mine = lane < ENT_CHAIN_BLOCKS && blk < nBlocks && rec->run;
+        const uint32_t n = mine ? nseqArr[blk] : 0u;
+        // stage the tables of the group's chained blocks, the whole warp on each (16 bytes per lane per step)
+        for (uint32_t run = __ballot_sync(B2Z_FULL, mine); run; run &= run - 1u) {
+            const uint32_t j = (uint32_t)__ffs((int)run) - 1u;
+            const uint4* s4 = reinterpret_cast<const uint4*>(&reinterpret_cast<const EntRec*>(scratch + (size_t)(blk0 + j) * ENT_SCRATCH_STRIDE)->tab);
             uint4* d4 = reinterpret_cast<uint4*>(&tabs[j]);
             for (uint32_t i = lane; i < sizeof(EntTables) / 16u; i += 32) d4[i] = s4[i];
         }
-        if (lane < ENT_CHAIN_BLOCKS)
-            nsq[lane] = lane < nb && reinterpret_cast<const EntRec*>(scratch + (size_t)(blk0 + lane) * ENT_SCRATCH_STRIDE)->run ? nseqArr[blk0 + lane] : 0u;
         __syncwarp();
-        const uint32_t blk = blk0 + b;
-        const bool mine = b < nb;
-        const uint32_t n = mine ? nsq[b] : 0u;
-        EntRec* rec = reinterpret_cast<EntRec*>(scratch + (size_t)(mine ? blk : blk0) * ENT_SCRATCH_STRIDE);
-        uint32_t* words = reinterpret_cast<uint32_t*>(scratch + (size_t)blk * ENT_SCRATCH_STRIDE + sizeof(EntRec));
-        const uint16_t* stT = tabs[mine ? b : 0].state + (t == 0 ? 0u : (t == 1 ? ENT_ST_OF : ENT_ST_ML));
-        const uint2* syT = tabs[mine ? b : 0].sym + (t == 0 ? 0u : (t == 1 ? ENT_SY_OF : ENT_SY_ML));
-        const uint32_t nMax = warp_max(n);
-        uint32_t state = 0;
-        for (uint32_t k0 = 0; k0 < nMax; k0 += ENT_CHAIN_SEQS) {
-            // codes of walk steps k0 .. k0 + 47 of every block (sequence n - 1 - k)
-            uint64_t v[ENT_CHAIN_LOADS];
+        E_TICK(E2C_STAGE);
+        const EntTables* tb = &tabs[mine ? lane : 0u];
+        const uint16_t* stL = tb->state; const uint16_t* stO = tb->state + ENT_ST_OF; const uint16_t* stM = tb->state + ENT_ST_ML;
+        const uint2* sy = tb->sym;
+        uint4* w4 = reinterpret_cast<uint4*>(scratch + (size_t)(mine ? blk : blk0) * ENT_SCRATCH_STRIDE + sizeof(EntRec));
+        const int32_t nV = (int32_t)((n + 3u) >> 2), last = (int32_t)n - 1;
+        const uint32_t rounds = warp_max(((uint32_t)nV + ENT_CHAIN_VECS - 1u) / ENT_CHAIN_VECS);
+        uint4 cur[ENT_CHAIN_VECS];
 #pragma unroll
-            for (uint32_t m = 0; m < ENT_CHAIN_LOADS; m++) {
-                const uint32_t j = lane + 32u * m, bj = j / ENT_CHAIN_SEQS, k = k0 + j % ENT_CHAIN_SEQS, nj = nsq[bj];
-                v[m] = k < nj ? seqs[(size_t)(blk0 + bj) * B2Z_MAXSEQ + (nj - 1u - k)] : 0ull;
-            }
+        for (int32_t m = 0; m < ENT_CHAIN_VECS; m++) { const int32_t q = nV - 1 - m; cur[m] = q >= 0 ? w4[q] : make_uint4(0, 0, 0, 0); }
+        uint32_t sL = 0, sO = 0, sM = 0;
+        if (n) {                                                 // the last sequence sets the initial states
+            const uint32_t e = (uint32_t)last & 3u;
+            const uint32_t c = e == 0 ? cur[0].x : (e == 1 ? cur[0].y : (e == 2 ? cur[0].z : cur[0].w));
+            sL = fse_first_state(stL, sy[c & 255u]);
+            sO = fse_first_state(stO, sy[ENT_SY_OF + ((c >> 8) & 255u)]);
+            sM = fse_first_state(stM, sy[ENT_SY_ML + (c >> 16)]);
+        }
+        E_TICK(E2C_LOAD);
+        for (uint32_t r = 0; r < rounds; r++) {
+            const int32_t q0 = nV - 1 - (int32_t)(r * ENT_CHAIN_VECS);
+            uint4 nxt[ENT_CHAIN_VECS];
 #pragma unroll
-            for (uint32_t m = 0; m < ENT_CHAIN_LOADS; m++) {
-                const uint32_t j = lane + 32u * m;
-                const uint64_t s = v[m];
-                codes[j / ENT_CHAIN_SEQS][j % ENT_CHAIN_SEQS] = s ? ll_code(B2Z_SEQ_LL(s)) | (highbit32(B2Z_SEQ_OFFBASE(s)) << 8) | (ml_code(B2Z_SEQ_ML(s) - 3u) << 16) : 0u;
+            for (int32_t m = 0; m < ENT_CHAIN_VECS; m++) {
+                const int32_t q = q0 - ENT_CHAIN_VECS - m;
+                nxt[m] = q >= 0 ? w4[q] : make_uint4(0, 0, 0, 0);
             }
-            __syncwarp();
-            const uint32_t kEnd = nMax - k0 < ENT_CHAIN_SEQS ? nMax - k0 : ENT_CHAIN_SEQS;
-            for (uint32_t kk = 0; kk < kEnd; kk++) {
-                const uint32_t k = k0 + kk;
-                const bool act = k < n;
-                uint32_t bits = 0, nbits = 0;
-                if (act) {
-                    const uint32_t sym = (codes[b][kk] >> (8u * t)) & 255u;
-                    const uint2 e = syT[sym];
-                    if (k == 0) {                                   // the last sequence sets the initial state
-                        const uint32_t nb0 = (e.x + (1u << 15)) >> 16;
-                        state = stT[(((nb0 << 16) - e.x) >> nb0) + e.y];
-                    } else {
-                        nbits = (state + e.x) >> 16; bits = state & ((1u << nbits) - 1u);
-                        state = stT[(state >> nbits) + e.y];
+            E_TICK(E2C_LOAD);
+#pragma unroll
+            for (int32_t m = 0; m < ENT_CHAIN_VECS; m++) {
+                const int32_t q = q0 - m;
+                if (q < 0) continue;
+                uint32_t w[4] = { cur[m].x, cur[m].y, cur[m].z, cur[m].w };
+#pragma unroll
+                for (int32_t e = 3; e >= 0; e--) {
+                    const int32_t i = 4 * q + e;
+                    if (i < last) {
+                        const uint32_t c = w[e];
+                        const uint2 eL = sy[c & 255u], eO = sy[ENT_SY_OF + ((c >> 8) & 255u)], eM = sy[ENT_SY_ML + (c >> 16)];
+                        uint32_t nL, nO, nM;
+                        const uint32_t bO = fse_step(stO, eO, sO, nO), bM = fse_step(stM, eM, sM, nM), bL = fse_step(stL, eL, sL, nL);
+                        w[e] = bO | (bM << nO) | (bL << (nO + nM)) | ((nO + nM + nL) << 26);
+                    } else if (i == last) {
+                        w[e] = 0;
                     }
                 }
-                // lane 3b gathers OF (3b+1) and ML (3b+2) and writes OF | ML | LL with the bit count on top
-                const uint32_t oB = __shfl_down_sync(B2Z_FULL, bits, 1), oN = __shfl_down_sync(B2Z_FULL, nbits, 1);
-                const uint32_t mB = __shfl_down_sync(B2Z_FULL, bits, 2), mN = __shfl_down_sync(B2Z_FULL, nbits, 2);
-                if (act && t == 0) words[n - 1u - k] = oB | (mB << oN) | (bits << (oN + mN)) | ((oN + mN + nbits) << 26);
+                cur[m] = make_uint4(w[0], w[1], w[2], w[3]);
             }
-            __syncwarp();
+            E_TICK(E2C_STEP);
+#pragma unroll
+            for (int32_t m = 0; m < ENT_CHAIN_VECS; m++) {
+                const int32_t q = q0 - m;
+                if (q >= 0) w4[q] = cur[m];
+                cur[m] = nxt[m];
+            }
+            E_TICK(E2C_STORE);
         }
-        if (n) rec->fin[t] = (uint16_t)state;
+        if (n) { rec->fin[0] = (uint16_t)sL; rec->fin[1] = (uint16_t)sO; rec->fin[2] = (uint16_t)sM; }
         __syncwarp();
+        E_TICK(E2C_STORE);
     }
+    E_CLOCKS_FLUSH(E1C_N, E2C_N);
 }
 
 // ---------------------------------------------------------------- E3: the sequence bitstream, one warp per block
@@ -851,6 +929,15 @@ zstd_enc_seqbits_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGe
 }
 
 #ifndef B2Z_CUEMU
+#ifdef B2Z_E_CLOCKS
+// the per-phase cycle sums of the E1 and E2 warps since the last call (E1C_* order, then E2C_*); clears them
+extern "C" int b200z_e_clocks(unsigned long long* out) {
+    static const unsigned long long zero[E1C_N + E2C_N] = {};
+    cudaError_t e = cudaMemcpyFromSymbol(out, e_clocks, sizeof(e_clocks));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(e_clocks, zero, sizeof(e_clocks));
+    return (int)e;
+}
+#endif
 void launch_zstd_enc_entropy(const uint8_t* src, uint64_t srcSize, const EncGeom& g,
                              const uint64_t* seqs, const uint32_t* nseq, const uint8_t* lits, const uint32_t* nlit,
                              uint8_t* slots, uint32_t* slotSize, uint8_t* scratch, uint32_t nBlocks, uint32_t smCount, cudaStream_t st) {
@@ -859,14 +946,17 @@ void launch_zstd_enc_entropy(const uint8_t* src, uint64_t srcSize, const EncGeom
     const uint32_t cap = smCount * 16u;
     if (grid > cap) grid = cap;
     zstd_enc_tables_kernel<<<grid, B2Z_ENT_WARPS * 32, 0, st>>>(src, srcSize, g, seqs, nseq, lits, nlit, slots, slotSize, scratch, nBlocks);
-    zstd_enc_chains_kernel<<<(nBlocks + ENT_CHAIN_BLOCKS - 1) / ENT_CHAIN_BLOCKS, 32, 0, st>>>(seqs, nseq, scratch, nBlocks);
+    cudaFuncSetAttribute(zstd_enc_chains_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ENT_CHAIN_SMEM);
+    cudaFuncSetAttribute(zstd_enc_chains_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    zstd_enc_chains_kernel<<<(nBlocks + ENT_CHAIN_BLOCKS - 1) / ENT_CHAIN_BLOCKS, 32, ENT_CHAIN_SMEM, st>>>(nseq, scratch, nBlocks);
     zstd_enc_seqbits_kernel<<<grid, B2Z_ENT_WARPS * 32, 0, st>>>(src, srcSize, g, seqs, nseq, slots, slotSize, scratch, nBlocks);
 }
 #else
 // Host emulation (tests/cuemu): the emulator's stage E entry launches zstd_enc_entropy_kernel once, over 4-warp CTAs of the
 // blocks.  Stage E is three launches with scratch between them, so under the emulator that entry's first thread runs E1, E2
-// and E3 in turn over every block -- the launches launch_zstd_enc_entropy makes -- with scratch of its own, and counts their
-// collectives as its own.  Every other thread returns at once.
+// and E3 in turn over every block -- the launches launch_zstd_enc_entropy makes, E2 as one-warp CTAs of ENT_CHAIN_BLOCKS blocks
+// with ENT_CHAIN_SMEM bytes of dynamic shared memory -- with scratch of its own, and counts their collectives as its own.  Every
+// other thread returns at once.
 inline void zstd_enc_entropy_kernel(const uint8_t* src, uint64_t srcSize, EncGeom g, const uint64_t* seqs, const uint32_t* nseq,
                                     const uint8_t* lits, const uint32_t* nlit, uint8_t* slots, uint32_t* slotSize, uint32_t nBlocks) {
     if (blockIdx.x != 0 || threadIdx.x != 0 || !nBlocks) return;
@@ -875,7 +965,7 @@ inline void zstd_enc_entropy_kernel(const uint8_t* src, uint64_t srcSize, EncGeo
     uint8_t* const scratch = buf.data() + ((16u - ((uintptr_t)buf.data() & 15u)) & 15u);
     const dim3 grid((nBlocks + B2Z_ENT_WARPS - 1) / B2Z_ENT_WARPS), block(B2Z_ENT_WARPS * 32);
     uint64_t c = cuemu::launch(grid, block, 0, [&] { zstd_enc_tables_kernel(src, srcSize, g, seqs, nseq, lits, nlit, slots, slotSize, scratch, nBlocks); });
-    c += cuemu::launch(dim3((nBlocks + ENT_CHAIN_BLOCKS - 1) / ENT_CHAIN_BLOCKS), dim3(32), 0, [&] { zstd_enc_chains_kernel(seqs, nseq, scratch, nBlocks); });
+    c += cuemu::launch(dim3((nBlocks + ENT_CHAIN_BLOCKS - 1) / ENT_CHAIN_BLOCKS), dim3(32), ENT_CHAIN_SMEM, [&] { zstd_enc_chains_kernel(nseq, scratch, nBlocks); });
     c += cuemu::launch(grid, block, 0, [&] { zstd_enc_seqbits_kernel(src, srcSize, g, seqs, nseq, slots, slotSize, scratch, nBlocks); });
     cuemu::blk() = outer;                                        // each launch leaves the emulator without a current CTA
     outer->collectives += c;
