@@ -684,7 +684,7 @@ int b200z_lzma2_compress_device(b200z_ctx* ctx, const void* d_src, size_t srcSiz
     { const int prc = lz2_check_props(ctx); if (prc) return prc; }
     if ((uintptr_t)d_src & 15u) return fail(ctx, B200Z_E_PARAM, "device source must be 16-byte aligned%s");
     if (dstCap < b200z_lzma2_compress_bound(ctx, srcSize)) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_lzma2_compress_bound%s");
-    if (dictProp) *dictProp = (ctx->geom.frameLog - 12u) * 2u;           // dictionary = frame size (Lzma2Enc_WriteProperties, Lzma2Enc.c:671)
+    if (dictProp) *dictProp = lzma2_dict_prop(ctx->geom.frameLog);     // dictionary = frame size
     CU(cudaSetDevice(ctx->device));
     if (srcSize == 0) {                                                  // the end marker alone
         CU(cudaMemsetAsync(d_dst, 0, 1, ctx->stream));
@@ -717,7 +717,7 @@ int b200z_lzma2_compress_host(b200z_ctx* ctx, const void* src, size_t srcSize, v
     if (!ctx || !dstSize || (!src && srcSize) || !dst) return B200Z_E_PARAM;
     { const int prc = lz2_check_props(ctx); if (prc) return prc; }
     if (dstCap < b200z_lzma2_compress_bound(ctx, srcSize)) return fail(ctx, B200Z_E_DSTSIZE, "dstCap < b200z_lzma2_compress_bound%s");
-    if (dictProp) *dictProp = (ctx->geom.frameLog - 12u) * 2u;
+    if (dictProp) *dictProp = lzma2_dict_prop(ctx->geom.frameLog);
     if (!srcSize) { *(uint8_t*)dst = 0; *dstSize = 1; return 0; }
     CU(cudaSetDevice(ctx->device));
     const uint64_t F = 1ull << ctx->geom.frameLog;

@@ -69,8 +69,8 @@ struct DecCounts { uint32_t nFrames, nBlocks, status, nUnits; uint64_t srcUsed; 
 // One walk for the D0 prepass (zstd_dec.cu reads through its Src) and the host queries (zstd_dec_api.cu, through HostBytes).  A
 // reader has u8 / le24 / le32: little-endian values at a byte offset.
 #define B2Z_ZSTD_MAGIC 0xFD2FB528u
-#define B2Z_DERR_TRUNCATED 32u       // the walk only: the bytes end inside a frame.  D0 reports it as B2Z_DERR_CORRUPT; a host query
-                                     // over a stream read piece by piece waits for more bytes
+#define B2Z_DERR_TRUNCATED 32u       // the header walks only (and lzma2_chunk): the bytes end inside a frame.  D0 reports it as
+                                     // B2Z_DERR_CORRUPT; a host query over a stream read piece by piece waits for more bytes
 
 struct HostBytes {                   // bytes past the end read as 0, as past the end of the device's Src
     const uint8_t* p; uint64_t size;

@@ -16,7 +16,6 @@ int lz2_status_to_rc(b200z_ctx* ctx, uint32_t status) {
 
 extern "C" {
 
-// Lzma2Decoder.cpp:40-48 / Lzma2Dec.c:29-31: dictionary size from the 1-byte coder property
 int b200z_lzma2_stream_info(const void* src, size_t srcSize, uint64_t* contentSize, uint32_t* nBlocks, size_t* srcUsed) {
     if (!src && srcSize) return B200Z_E_PARAM;
     Lz2Counts c;
@@ -38,29 +37,15 @@ int b200z_lzma2_stream_prefix(const void* srcv, size_t srcSize, uint64_t maxCont
     uint32_t nb = 0, nbAtBoundary = 0, needInit = 0xE0;
     int end = 0, rc = B200Z_OK;
     while (ip < srcSize) {
-        const uint32_t ctl = src[ip];
-        if (ctl == 0) { boundary = ip + 1; boundaryTotal = total; nbAtBoundary = nb; end = 1; break; }
-        uint64_t hdr, pack, unpack; bool reset;
-        if (ctl <= 2) {
-            if (ip + 3 > srcSize) break;
-            hdr = 3; pack = unpack = (((uint64_t)src[ip + 1] << 8) | src[ip + 2]) + 1; reset = ctl == 1;
-            if (ctl == 1) needInit = 0xC0; else if (needInit == 0xE0) { rc = B200Z_E_CORRUPT; break; }
-        } else {
-            if (ctl < 0x80 || ctl < needInit) { rc = B200Z_E_CORRUPT; break; }
-            needInit = 0;
-            const uint32_t mode = (ctl >> 5) & 3u;
-            hdr = 5 + (mode >= 2 ? 1 : 0);
-            if (ip + hdr > srcSize) break;
-            unpack = ((((uint64_t)ctl & 0x1F) << 16) | ((uint64_t)src[ip + 1] << 8) | src[ip + 2]) + 1;
-            pack = (((uint64_t)src[ip + 3] << 8) | src[ip + 4]) + 1;
-            reset = mode == 3;
-        }
-        if (reset) {                                            // everything before this header is whole blocks
+        const Lz2Chunk ch = lzma2_chunk(src + ip, srcSize - ip, needInit);
+        if (ch.status) { if (ch.status == B2Z_DERR_CORRUPT) rc = B200Z_E_CORRUPT; break; }         // cut off: wait for more bytes
+        if (ch.kind == LZ2_CHUNK_END) { boundary = ip + 1; boundaryTotal = total; nbAtBoundary = nb; end = 1; break; }
+        if (ch.reset) {                                         // everything before this header is whole blocks
             boundary = ip; boundaryTotal = total; nbAtBoundary = nb; nb++;
             if (nbAtBoundary && boundaryTotal >= maxContent) break;
         }
-        if (ip + hdr + pack > srcSize) break;
-        total += unpack; ip += hdr + pack;
+        if (ch.hdr + ch.pack > srcSize - ip) break;
+        total += ch.unpack; ip += ch.hdr + ch.pack;
     }
     if (usedBytes) *usedBytes = (size_t)boundary;
     if (contentSize) *contentSize = boundaryTotal;
@@ -75,7 +60,7 @@ int b200z_lzma2_decompress_device(b200z_ctx* ctx, const void* d_src, size_t srcS
     *dstSize = 0;
     if (dictProp > 40) return fail(ctx, B200Z_E_UNSUPPORTED, "LZMA2: dictionary property above 40%s");
     if (!srcSize) return fail(ctx, B200Z_E_CORRUPT, "LZMA2: empty stream (no end marker)%s");
-    const uint32_t dictSize = dictProp == 40 ? 0xFFFFFFFFu : ((2u | (dictProp & 1u)) << (dictProp / 2u + 11u));
+    const uint32_t dictSize = lzma2_dict_size(dictProp);
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     Arena& aBlocks = ctx->decScratch[6]; Arena& aCounts = ctx->decScratch[7];

@@ -127,32 +127,17 @@ lzma2_decode_kernel(const uint8_t* __restrict__ src, const Lz2Block* __restrict_
                         if (rc.ip != rc.end || rc.code != 0) { op = OP_ERROR; break; }
                     }
                     if (hp >= blkEnd) { op = (pos == blkSize) ? OP_END : OP_ERROR; break; }
-                    const uint32_t ctl = hp[0];
-                    if (ctl <= 2) {                                 // 0 cannot occur before blkEnd (the walk stops there)
-                        if (ctl == 0) { op = OP_ERROR; break; }
-                        if (ctl == 1) needInit = 0xC0; else if (needInit == 0xE0) { op = OP_ERROR; break; }
-                        const uint32_t n = (((uint32_t)hp[1] << 8) | hp[2]) + 1u;
-                        if (n > blkSize - pos) { op = OP_ERROR; break; }
-                        rawSrc = hp + 3; hp += 3 + n;
-                        op = OP_RAW; a = n; d = pos;
-                        pos += n; chunkEnd = pos;
-                        break;
-                    }
-                    if (ctl < 0x80 || ctl < needInit) { op = OP_ERROR; break; }
-                    needInit = 0;
-                    const uint32_t unpack = (((ctl & 0x1Fu) << 16) | ((uint32_t)hp[1] << 8) | hp[2]) + 1u;
-                    const uint32_t pack = (((uint32_t)hp[3] << 8) | hp[4]) + 1u;
-                    const uint32_t mode = (ctl >> 5) & 3u;
-                    hp += 5;
-                    if (mode >= 2) {
-                        uint32_t pr = *hp++;
-                        lc = pr % 9u; pr /= 9u; pb = pr / 5u; lp = pr % 5u;     // validated by the walk
-                        litCount = 0x300u << (lc + lp);
-                    }
-                    if (unpack > blkSize - pos || pack < 5) { op = OP_ERROR; break; }
-                    rc.base = hp; rc.ip = 0; rc.end = pack; hp += pack;
-                    chunkEnd = pos + unpack; pendingInit = true;
-                    if (mode >= 1) { state = 0; rep0 = rep1 = rep2 = rep3 = 0; op = OP_RESET; a = P_LIT + litCount; break; }
+                    // an end marker cannot occur before blkEnd (the walk stops there)
+                    const Lz2Chunk ch = lzma2_chunk(hp, (uint64_t)(blkEnd - hp), needInit);
+                    if (ch.status || ch.kind == LZ2_CHUNK_END || ch.unpack > blkSize - pos) { op = OP_ERROR; break; }
+                    const uint8_t* const payload = hp + ch.hdr;
+                    hp = payload + ch.pack;
+                    if (ch.kind == LZ2_CHUNK_STORED) { rawSrc = payload; op = OP_RAW; a = ch.unpack; d = pos; pos += ch.unpack; chunkEnd = pos; break; }
+                    if (ch.mode >= 2) { lc = ch.lc; lp = ch.lp; pb = ch.pb; litCount = 0x300u << (lc + lp); }
+                    if (ch.pack < 5) { op = OP_ERROR; break; }
+                    rc.base = payload; rc.ip = 0; rc.end = ch.pack;
+                    chunkEnd = pos + ch.unpack; pendingInit = true;
+                    if (ch.mode >= 1) { state = 0; rep0 = rep1 = rep2 = rep3 = 0; op = OP_RESET; a = P_LIT + litCount; break; }
                 }
                 if (pendingInit) {                                  // range decoder start: 0x00 + 4 bytes big-endian (LzmaDec.c:987-998)
                     pendingInit = false; inChunk = true;

@@ -115,21 +115,7 @@ lzma2_enc_range_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncGeo
 
     auto chunk_close = [&](uint32_t pos) {
         for (int i = 0; i < 5; i++) rce_shift_low(e);
-        const uint32_t unpack = pos - chunkPos, pack = e.op - chunkOut - hdr;
-        uint8_t* h = e.out + chunkOut;
-        if (pack + 2u >= unpack) {                                  // store the chunk uncompressed
-            h[0] = needDict ? 1 : 2; h[1] = (uint8_t)((unpack - 1u) >> 8); h[2] = (uint8_t)(unpack - 1u);
-            const uint8_t* s = base + chunkPos;
-            for (uint32_t i = 0; i < unpack; i++) h[3u + i] = __ldg(s + i);
-            e.op = chunkOut + 3u + unpack;
-            needDict = false; needState = true;
-        } else {
-            const uint32_t mode = needDict ? 3u : (needProps ? 2u : (needState ? 1u : 0u));
-            h[0] = (uint8_t)(0x80u | (mode << 5) | ((unpack - 1u) >> 16)); h[1] = (uint8_t)((unpack - 1u) >> 8); h[2] = (uint8_t)(unpack - 1u);
-            h[3] = (uint8_t)((pack - 1u) >> 8); h[4] = (uint8_t)(pack - 1u);
-            if (mode >= 2u) h[5] = (uint8_t)props;
-            needDict = needProps = needState = false;
-        }
+        lzma2_chunk_write(e.out, e.op, chunkOut, hdr, base + chunkPos, pos - chunkPos, props, needDict, needProps, needState);
         open = false;
     };
     auto chunk_step = [&](uint32_t pos) {                           // before every packet
@@ -326,21 +312,7 @@ lzma2_enc_range32_kernel(const uint8_t* __restrict__ src, uint64_t srcSize, EncG
 
     auto chunk_close = [&](uint32_t pos) {                                              // (queue empty)
         for (int i = 0; i < 5; i++) rce32_shift_low(e);
-        const uint32_t unpack = pos - chunkPos, pack = e.op - chunkOut - hdr;
-        uint8_t* h = e.out + chunkOut;
-        if (pack + 2u >= unpack) {                                                      // store the chunk uncompressed
-            h[0] = needDict ? 1 : 2; h[1] = (uint8_t)((unpack - 1u) >> 8); h[2] = (uint8_t)(unpack - 1u);
-            const uint8_t* s = base + chunkPos;
-            for (uint32_t i = 0; i < unpack; i++) h[3u + i] = __ldg(s + i);
-            e.op = chunkOut + 3u + unpack;
-            needDict = false; needState = true;
-        } else {
-            const uint32_t mode = needDict ? 3u : (needProps ? 2u : (needState ? 1u : 0u));
-            h[0] = (uint8_t)(0x80u | (mode << 5) | ((unpack - 1u) >> 16)); h[1] = (uint8_t)((unpack - 1u) >> 8); h[2] = (uint8_t)(unpack - 1u);
-            h[3] = (uint8_t)((pack - 1u) >> 8); h[4] = (uint8_t)(pack - 1u);
-            if (mode >= 2u) h[5] = (uint8_t)props;
-            needDict = needProps = needState = false;
-        }
+        lzma2_chunk_write(e.out, e.op, chunkOut, hdr, base + chunkPos, pos - chunkPos, props, needDict, needProps, needState);
         open = false;
     };
     auto chunk_open = [&](uint32_t pos) {                                               // (queue empty)

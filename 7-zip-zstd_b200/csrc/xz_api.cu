@@ -282,7 +282,7 @@ int b200z_xz_decompress_host(b200z_ctx* ctx, const void* srcv, size_t n, void* d
     size_t o = 0;
     for (const auto& b : blocks) {
         if (b.packSize < 1 || s[b.packOff + b.packSize - 1] != 0) return fail(ctx, B200Z_E_CORRUPT, "xz: Block without an end marker%s");
-        if (b.packSize > 1 && s[b.packOff] != 0x01 && s[b.packOff] < 0xE0) return fail(ctx, B200Z_E_CORRUPT, "xz: Block does not start with a dictionary reset%s");
+        if (b.packSize > 1 && !b2z::lzma2_is_reset(s[b.packOff])) return fail(ctx, B200Z_E_CORRUPT, "xz: Block does not start with a dictionary reset%s");
         memcpy(lz.data() + o, s + b.packOff, (size_t)b.packSize - 1); o += (size_t)b.packSize - 1;
     }
     lz[o++] = 0;

@@ -182,7 +182,7 @@ int64_t emu_lzma2_decode(const uint8_t* src, uint64_t srcSize, uint32_t dictProp
     cuemu::launch(dim3(1), dim3(32), 0, [&] { lzma2_walk_kernel(src, srcSize, blocks.data(), (uint32_t)blocks.size(), &counts); });
     if (counts.status) return -(int64_t)counts.status;
     if (counts.total > dstCap) return -100;
-    const uint32_t dictSize = dictProp == 40 ? 0xFFFFFFFFu : ((2u | (dictProp & 1u)) << (dictProp / 2u + 11u));
+    const uint32_t dictSize = lzma2_dict_size(dictProp);
     const uint32_t litCount = 0x300u << counts.maxLcLp;
     std::vector<uint16_t> spill(glit ? (size_t)counts.nBlocks * litCount : 1);
     if (counts.nBlocks) {

@@ -595,5 +595,7 @@ def header_only_stream():
 
 def test_block_of_4gib_is_unsupported(pkg):
     L = _lib(pkg)
-    rc, cs, nb, _ = stream_info(L, header_only_stream())
+    comp = header_only_stream()
+    rc, cs, nb, _ = stream_info(L, comp)
     assert rc == -6 and nb == 1 and cs >= 1 << 32
+    assert stream_prefix(L, comp) == (0, len(comp), 2049 << 21, 1, 1)     # the streaming cut leaves the limit to the decoder

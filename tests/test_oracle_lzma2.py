@@ -96,14 +96,21 @@ def test_corruption_parity_with_reference():
 
 def test_chunk_header_rules_host_walk_and_oracle():
     """Lzma2Dec_UpdateState's needInitLevel rule and property checks (C/Lzma2Dec.c:97-165): the host walk
-    (b200z_lzma2_stream_info) and the oracle decoder reject the same malformed chunk sequences."""
+    (b200z_lzma2_stream_info) and the oracle decoder reject the same malformed chunk sequences; the streaming cut
+    (b200z_lzma2_stream_prefix) rejects those of them that are not merely cut short."""
     import ctypes
     lib = ctypes.CDLL(os.path.join(H.ROOT, "7-zip-zstd_b200", "libb200z.so"))
     lib.b200z_lzma2_stream_info.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_size_t)]
+    lib.b200z_lzma2_stream_prefix.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_uint64, ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_uint64),
+                                              ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_int)]
 
     def walk(b):
         buf = ctypes.create_string_buffer(b, len(b)); cs, nb, used = ctypes.c_uint64(), ctypes.c_uint32(), ctypes.c_size_t()
         return lib.b200z_lzma2_stream_info(buf, len(b), ctypes.byref(cs), ctypes.byref(nb), ctypes.byref(used)), cs.value, nb.value, used.value
+
+    def prefix(b):
+        buf = ctypes.create_string_buffer(b, len(b)); used, cs, nb, ended = ctypes.c_size_t(), ctypes.c_uint64(), ctypes.c_uint32(), ctypes.c_int()
+        return lib.b200z_lzma2_stream_prefix(buf, len(b), 1 << 62, ctypes.byref(used), ctypes.byref(cs), ctypes.byref(nb), ctypes.byref(ended))
 
     raw = lambda ctl, payload: bytes([ctl, (len(payload) - 1) >> 8, (len(payload) - 1) & 0xFF]) + payload
     good = raw(1, b"hello") + raw(2, b" world") + b"\x00"
@@ -123,7 +130,9 @@ def test_chunk_header_rules_host_walk_and_oracle():
         bytes([0xE0, 0, 0, 0, 4, 225]) + bytes(5) + b"\x00",   # property byte out of range
         bytes([0xE0, 0, 0, 0, 4, 4 * 9 + 8 + 0]) + bytes(5) + b"\x00",   # lc 8 + lp 4 > 4
     ]
+    cut_short = {b"", raw(1, b"x"), raw(1, b"x")[:-1]}       # a stream read piece by piece waits for more bytes here
     for b in bad:
         assert walk(b)[0] == -5, b
+        assert prefix(b) == (0 if b in cut_short else -5), b
         with pytest.raises(ValueError):
             H.oracle_lzma2_decompress(b, 64, 0)
